@@ -1272,6 +1272,12 @@ int run_experiment_chunk(void *array, uint64_t num_trials, size_t stride, const 
 
         e = cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st);
         if (e != cudaSuccess) { rc = cuda_fail(e, "H2D"); goto done; }
+        // the arena is reused between calls and many kernels (M/M/1, M/M/c, ...) write no counters: without this the
+        // caller's counters field would receive whatever an earlier call left at these addresses
+        if (want_counters) {
+            e = cudaMemsetAsync(job.counters, 0, cnt_bytes, st);
+            if (e != cudaSuccess) { rc = cuda_fail(e, "counters memset"); goto done; }
+        }
         rc = cimba_b200_launch(&job, st);
         if (rc != CIMBA_B200_OK) goto done;
         e = cudaMemcpyAsync(h_out, d_out, out_bytes + (want_counters ? cnt_bytes : 0), cudaMemcpyDeviceToHost, st);

@@ -288,6 +288,8 @@ int cimba_b200_summarize_weighted(const double *x, const double *w, uint64_t n,
 /* cmb_wtdsummary_merge (src/cmb_wtdsummary.c:152-194) over n device-resident rows of that
  * format (one per trial) into one row: the per-GPU step before the NCCL all-gather. */
 int cimba_b200_merge_weighted_rows(const uint64_t *rows, uint64_t n, uint64_t *out_row, void *stream);
+/* All three reductions refuse an empty input: num_trials / n = 0 returns CIMBA_B200_EINVAL, launches nothing and leaves
+ * the output untouched (an empty summary is what *_initialize gives on the host). */
 
 /* ------------------------------------------------------------------------
  * Host-buffer interface = the cimba_run_experiment() replacement.

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from oracle_libs import rng_draws, run_trials, trace_trial
+from param_cases import TABLE
 
 KAT_SEED = 0x34F05C64D7AD598F
 
@@ -266,6 +267,24 @@ def test_port_equals_live_reference(port, ref, model, arr, srv, servers):
     ra, ka, ta = trace_trial(ref, "ref", model, servers, 99, 3000 if model in (0, 1, 2, 9) else (15 if model == 7 else 800), arr, srv, 9000)
     rb, kb, tb = trace_trial(port, "port", model, servers, 99, 3000 if model in (0, 1, 2, 9) else (15 if model == 7 else 800), arr, srv, 9000)
     assert ka == kb and ta == tb and ra.key() == rb.key()
+
+
+@pytest.mark.parametrize("model,servers,rho", [(m, TABLE[m][0], "load") for m in TABLE if m not in (16, 17, 19)]
+                         + [(2, 8, "load"), (0, 1, "repair"), (1, 1, "repair"), (2, 3, "repair"), (2, 8, "repair"),
+                            (9, 1, "repair")])
+def test_port_equals_live_reference_at_per_trial_parameters(port, ref, model, servers, rho):
+    """tests/param_cases.py's table (each trial its own arr_mean and srv_mean, srv_mean never 1.0, time scales 1e-3 .. 1234.5):
+    the port, which the GPU suite checks every kernel against, is the reference at every parameter set of it."""
+    from param_cases import RHO, RHO_REPAIR, oracle, per_trial_params
+    if ref is None:
+        pytest.skip("oracle/_ref not built here (no reference sources)")
+    arr, srv = per_trial_params(model, servers=servers, rho=RHO if rho == "load" else RHO_REPAIR)
+    nobj = TABLE[model][1]
+    a = oracle(ref, "ref", model, servers, nobj, arr, srv)
+    b = oracle(port, "port", model, servers, nobj, arr, srv)
+    assert [x.key() for x in a] == [x.key() for x in b]
+    assert [(x.max_fel, x.max_queue) for x in a] == [(x.max_fel, x.max_queue) for x in b]
+    assert [x.counters() for x in a] == [x.counters() for x in b]
 
 
 def test_reference_pthread_executive_equals_serial(ref):
