@@ -31,6 +31,9 @@ namespace cimba_b200 {
 #ifndef MM1_COLD_BATCH
 #define MM1_COLD_BATCH 4       // parked lanes needed before the ziggurat slow path runs
 #endif
+#ifndef MM1_STEPS
+#define MM1_STEPS 2            // event steps per loop iteration (divides MM1_PARK_MASK + 1)
+#endif
 
 // 32-bit shared-window accesses: one address register, no generic->shared
 // conversion per access (the static-__shared__ form costs extra
@@ -114,7 +117,14 @@ mm1_kernel(const QueueArgs a)
     // unused raw draw remains when the trial ends.
     uint64_t u_next = 0u;
     double e_next = 0.0;                                // hot-path std exponential of u_next
+    uint32_t off_next = 0u;                             // u_next's ziggurat layer as a byte offset into exp_x
     uint32_t pops = 0u;
+    // (u & 0xff) * 8 as hi((u << 24) * 2^11): two IMADs instead of a shift and a mask
+    const auto refill = [&]() {
+        u_next = rng.next_imad();
+        off_next = imad_hi(imad_lo((uint32_t)u_next, IMAD_K2P24, 0u), IMAD_K2P11, 0u);
+        e_next = __dmul_rn(lds_f64(tab + off_next), __ull2double_rn(u_next));
+    };
 
     if (alive) {
         arr_mean = a.arr_mean[trial];
@@ -123,26 +133,26 @@ mm1_kernel(const QueueArgs a)
         t_arr = 0.0; k_arr = pack_key(1u, ACT_START);   // cmb_process_start(arrival), MM1_multi.c:107-108
         t_srv = 0.0; k_srv = pack_key(2u, ACT_START);   // cmb_process_start(service), :109-111
         issued = 2u;
-        u_next = rng.next();
-        e_next = __dmul_rn(lds_f64(tab + ((uint32_t)u_next & 0xffu) * 8u), __ull2double_rn(u_next));
+        refill();
     }
 
-    // lane state in one word: bit 0 alive, bit 1 parked (the look-ahead variate needs the
-    // ziggurat slow path), bit 2 the parked draw belongs to the arrival process
+    // lane state in one word: 1 running, 3 parked (the look-ahead variate needs the ziggurat
+    // slow path) in the service process, 7 parked in the arrival process, 0 finished
     uint32_t flags = alive ? 1u : 0u;
     uint32_t step = 0u;
 
-    while (__any_sync(FULL, flags & 1u)) {
+    // One event step.  A lane that is finished or parked runs it with every update predicated off, so the registers of a
+    // finished trial hold its results until they are written after the loop.
+    const auto event_step = [&]() {
         // ---------------- pop-min (cmi_hashheap_dequeue order: time asc, key asc)
-        const bool go0 = (flags & 3u) == 1u;           // alive and not parked
+        const bool go0 = flags == 1u;                   // alive and not parked
         const bool first_arr = (t_arr < t_srv) | ((t_arr == t_srv) & (k_arr < k_srv));
         const uint32_t key = first_arr ? k_arr : k_srv;
-        const uint32_t act = key & 3u;
         const bool go = go0 & (key != 0u);
-        const bool done = go0 & (key == 0u);            // event list ran dry
+        if (go0 & (key == 0u)) flags = 0u;              // event list ran dry: the trial is over
         const bool is_arr = go & first_arr;
         const bool is_srv = go & !first_arr;
-        const bool wake = act == ACT_WAKE_TIME;
+        const bool wake = (key & 3u) == ACT_WAKE_TIME;
         if (TRACE) {
             if (go && pops < a.trace_cap) {
                 a.trace_key[trial * a.trace_cap + pops] = key >> 2;
@@ -155,49 +165,35 @@ mm1_kernel(const QueueArgs a)
         // ---------------- arrival body (MM1_multi.c:58-66): back from hold -> put
         // Ring accesses are unconditional (a lane that does not put writes its private
         // scratch row instead): a select on the address is cheaper than a divergent region.
-        const uint32_t q_len = produced - served;
+        const uint32_t p0 = produced, s0 = served;
+        const uint32_t q_len = p0 - s0;
         const bool put = is_arr & wake;
         const bool put_far = put & (q_len >= (uint32_t)QUEUE_WINDOW);
-        sts_f64((put & !put_far) ? win + (produced & WMASK) * ROW : scratch, now);
-        if (put_far) {                                  // rare: beyond the on-chip window
-            if (spill != nullptr && q_len - QUEUE_WINDOW <= spill_mask) {
-                spill[produced & spill_mask] = now;
-            }
-            else {
-                status |= TRIAL_ERR_QUEUE_OVERFLOW;     // entry dropped: the trial is void from here on
-                dropped++;
-                served++;                               // keep produced - served = entries actually stored
-            }
-        }
+        sts_f64((put & !put_far) ? win + (p0 & WMASK) * ROW : scratch, now);
         if (put) produced++;
-        longest = max(longest, produced - served);
         // cmb_objectqueue_put -> cmb_resourceguard_signal(front guard): wake the server
-        const bool ring_bell = put & (k_srv == 0u);
-        if (ring_bell) {
+        if (put & (k_srv == 0u)) {
             issued++;
             t_srv = now;
             k_srv = pack_key(issued, ACT_WAKE_RESOURCE);
         }
 
         // ---------------- service body (MM1_multi.c:78-88)
-        const bool finished = is_srv & wake;            // back from the service hold
         const double new_sum = __dadd_rn(sum_wait, __dsub_rn(now, stamp));
-        if (finished) sum_wait = new_sum;
+        if (is_srv & wake) sum_wait = new_sum;          // back from the service hold
         // cmb_objectqueue_get: take the head, or wait at the front guard (slot stays empty)
-        const bool take = is_srv & (produced != served);
-        const uint32_t head_slot = win + (served & WMASK) * ROW;
+        const bool take = is_srv & (q_len != 0u);
+        const uint32_t head_slot = win + (s0 & WMASK) * ROW;
         const double head_stamp = lds_f64(head_slot);   // harmless when the ring is empty
-        if (take) stamp = head_stamp;
-        // (a warp-wide vote + branch around these six predicated-off instructions puts the vote on the critical path of
-        // every step)
-        if (take & (produced - served > (uint32_t)QUEUE_WINDOW)) {      // rare: refill the freed slot from HBM
-            sts_f64(head_slot, spill[(served + QUEUE_WINDOW) & spill_mask]);
+        if (take) {
+            stamp = head_stamp;
+            served++;
         }
-        if (take) served++;
+        const bool refill_far = take & (q_len > (uint32_t)QUEUE_WINDOW);
 
         // ---------------- hold: consume the look-ahead variate, insert the wake-up
         const bool draw = take | (is_arr & (produced < quota));
-        const bool hot = Sfc64::exp_is_hot(u_next);
+        const bool hot = off_next <= ZIG_EXP_MAX * 8u;  // Sfc64::exp_is_hot(u_next)
         const bool push = draw & hot;
         const double when = __dadd_rn(now, __dmul_rn(is_arr ? arr_mean : srv_mean, e_next));
         if (push) issued++;
@@ -206,22 +202,33 @@ mm1_kernel(const QueueArgs a)
         if (is_arr) { t_arr = t_new; k_arr = k_new; }
         if (is_srv) { t_srv = t_new; k_srv = k_new; }
         if (draw & !hot) flags = is_arr ? 7u : 3u;
-        if (push) {                                     // refill the look-ahead
-            u_next = rng.next();
-            e_next = __dmul_rn(lds_f64(tab + ((uint32_t)u_next & 0xffu) * 8u), __ull2double_rn(u_next));
-        }
+        if (push) refill();
 
-        // ---------------- rare paths
-        if (done) {
-            flags = 0u;
-            if (a.events)    a.events[trial] = issued;  // every scheduled event has been popped
-            if (a.objects)   a.objects[trial] = served - dropped;
-            if (a.t_end)     a.t_end[trial] = now;
-            if (a.sum_wait)  a.sum_wait[trial] = sum_wait;
-            if (a.status)    a.status[trial] = status | (issued > 0x3ffffff0u ? TRIAL_ERR_KEY_OVERFLOW : 0u);
-            if (a.max_queue) a.max_queue[trial] = longest;
+        // ---------------- rare: the queue reaches past the on-chip window
+        if (put_far | refill_far) {
+            if (refill_far) {                           // refill the freed slot from HBM
+                sts_f64(head_slot, spill[(s0 + QUEUE_WINDOW) & spill_mask]);
+            }
+            else if (spill != nullptr && q_len - QUEUE_WINDOW <= spill_mask) {
+                spill[p0 & spill_mask] = now;
+            }
+            else {
+                status |= TRIAL_ERR_QUEUE_OVERFLOW;     // entry dropped: the trial is void from here on
+                dropped++;
+                served++;                               // keep produced - served = entries actually stored
+            }
         }
-        if ((++step & MM1_PARK_MASK) != 0u) {
+        longest = max(longest, produced - served);
+    };
+
+    // MM1_STEPS event steps per iteration share one exit vote and one look at the parked set
+    while (__any_sync(FULL, flags & 1u)) {
+#pragma unroll
+        for (int i = 0; i < MM1_STEPS; i++) {
+            event_step();
+        }
+        step += MM1_STEPS;
+        if ((step & MM1_PARK_MASK) != 0u) {
             continue;                                   // look at the parked set every (MM1_PARK_MASK+1)-th step only
         }
         const unsigned pm = __ballot_sync(FULL, flags & 2u);
@@ -236,13 +243,21 @@ mm1_kernel(const QueueArgs a)
                     if (parked_is_arr) { t_arr = at; k_arr = pack_key(issued, ACT_WAKE_TIME); }
                     else               { t_srv = at; k_srv = pack_key(issued, ACT_WAKE_TIME); }
                     flags = 1u;
-                    u_next = rng.next();
-                    e_next = __dmul_rn(lds_f64(tab + ((uint32_t)u_next & 0xffu) * 8u), __ull2double_rn(u_next));
+                    refill();
                 }
             }
         }
     }
-    if (a.diag != nullptr && lane == 0u) {             // bench.py: loop iterations -> issued warp-instructions
+    // every update above is predicated on a running lane: the registers hold each trial's results
+    if (alive) {
+        if (a.events)    a.events[trial] = issued;      // every scheduled event has been popped
+        if (a.objects)   a.objects[trial] = served - dropped;
+        if (a.t_end)     a.t_end[trial] = now;
+        if (a.sum_wait)  a.sum_wait[trial] = sum_wait;
+        if (a.status)    a.status[trial] = status | (issued > 0x3ffffff0u ? TRIAL_ERR_KEY_OVERFLOW : 0u);
+        if (a.max_queue) a.max_queue[trial] = longest;
+    }
+    if (a.diag != nullptr && lane == 0u) {             // bench.py: event steps -> issued warp-instructions
         atomicAdd(a.diag, (unsigned long long)step);
         atomicAdd(a.diag + 1, 1ull);
     }

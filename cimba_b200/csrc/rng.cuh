@@ -66,6 +66,48 @@ constexpr double TWO_POW_64 = 18446744073709551616.0;
 constexpr double TWO_POW_63 = 9223372036854775808.0;
 constexpr double TWO_POW_M53 = 1.1102230246251565404e-16;
 
+#ifndef CMB_HOST_BUILD
+// Integer multipliers read from the constant bank.  ptxas rewrites a multiply by an immediate 1 or power of two as an add or a
+// shift (the half-rate ALU pipe); a constant-bank operand it cannot see into keeps the operation an IMAD (the FMA pipe).
+static __constant__ uint32_t imad_k[3] = {1u << 21, 1u << 24, 1u << 11};
+#define IMAD_K2P21 imad_k[0]
+#define IMAD_K2P24 imad_k[1]
+#define IMAD_K2P11 imad_k[2]
+
+__device__ __forceinline__ uint64_t u64_of(uint32_t lo, uint32_t hi)
+{
+    uint64_t r;
+    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
+    return r;
+}
+
+__device__ __forceinline__ void u32_of(uint64_t v, uint32_t &lo, uint32_t &hi)
+{
+    asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v));
+}
+
+__device__ __forceinline__ uint64_t imad_wide(uint32_t x, uint32_t y, uint64_t z)       // x * y + z, 64-bit
+{
+    uint64_t r;
+    asm("mad.wide.u32 %0, %1, %2, %3;" : "=l"(r) : "r"(x), "r"(y), "l"(z));
+    return r;
+}
+
+__device__ __forceinline__ uint32_t imad_lo(uint32_t x, uint32_t y, uint32_t z)         // low word of x * y + z
+{
+    uint32_t r;
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(x), "r"(y), "r"(z));
+    return r;
+}
+
+__device__ __forceinline__ uint32_t imad_hi(uint32_t x, uint32_t y, uint32_t z)         // high word of x * y, plus z
+{
+    uint32_t r;
+    asm("mad.hi.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(x), "r"(y), "r"(z));
+    return r;
+}
+#endif
+
 struct Sfc64 {
     uint64_t a, b, c, d;
 
@@ -93,6 +135,42 @@ struct Sfc64 {
 #endif
         c = ((c << 24) | (c >> 40)) + out;
         return out;
+    }
+
+    // The same step as next() with its shifts also on the FMA pipe, for a kernel whose ALU pipe is the busier one
+    // (mm1_kernel).  It is not the default: in the G/G/1 and M/M/c kernels and the static tier it measured slower on the H100.
+    __device__ __forceinline__ uint64_t next_imad()
+    {
+#if !defined(SFC64_NO_IMAD) && !defined(CMB_HOST_BUILD)
+        // The shifts run as IMAD on the FMA pipe instead of SHF on the half-rate ALU pipe, the busiest pipe of every event loop
+        // here; the additions and XORs stay on the ALU pipe as three-input IADD3 / LOP3.  Integer arithmetic is exact: the
+        // same values, bit for bit (define SFC64_NO_IMAD for the plain form).
+        //   b ^ (b >> 11)      = {b.lo ^ hi(b.lo * 2^21) ^ lo(b.hi * 2^21), b.hi ^ hi(b.hi * 2^21)}
+        //   c + (c << 3) = 9 c = c.lo * 9 (wide), + c.hi * 9 in the high word
+        //   rotl(c, 24)        = c.lo * 2^24 (wide) + {hi(c.hi * 2^24), lo(c.hi * 2^24)}   (no two terms share a bit)
+        const uint64_t out = a + b + d++;
+        uint32_t bl, bh, cl, ch;
+        u32_of(b, bl, bh);
+        u32_of(c, cl, ch);
+        {
+            uint32_t wl, wh;
+            u32_of(imad_wide(bh, IMAD_K2P21, 0ull), wl, wh);
+            a = u64_of(bl ^ imad_hi(bl, IMAD_K2P21, 0u) ^ wl, bh ^ wh);
+        }
+        {
+            uint32_t wl, wh;
+            u32_of(imad_wide(cl, 9u, 0ull), wl, wh);
+            b = u64_of(wl, imad_lo(ch, 9u, wh));
+        }
+        {
+            uint32_t wl, wh;
+            u32_of(imad_wide(ch, IMAD_K2P24, 0ull), wl, wh);
+            c = imad_wide(cl, IMAD_K2P24, 0ull) + u64_of(wh, wl) + out;
+        }
+        return out;
+#else
+        return next();
+#endif
     }
 
     // The inverse of next(): puts the last output back.  sfc64's state transition is a bijection

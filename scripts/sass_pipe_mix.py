@@ -2,9 +2,12 @@
 """Per-pipe instruction mix of a kernel's main loop, from the SASS of a built library (no GPU needed).
 
     python scripts/sass_pipe_mix.py cimba_b200/lib/libcimba_b200.so mm1_kernelILb0 [--list]
+        [--exclude START-END,...] [--steps N]
 
 The loop = the backward branch with the largest span (as scripts/sass_loop_stats.py); every instruction inside it is counted,
-rare blocks included.  Pipes as ncu's sm__inst_executed_pipe_* names them: alu (integer add / logic / shift / compare /
+rare blocks included, unless --exclude names address ranges (hex, both ends included, as --list prints them) to leave out:
+the rare blocks, so that what remains is the path most iterations take.  --steps N also prints the counts divided by N, for
+a loop whose body runs N event steps.  Pipes as ncu's sm__inst_executed_pipe_* names them: alu (integer add / logic / shift / compare /
 select - half rate), fma (IMAD*, FP32), fp64, xu (conversions, MUFU, POPC), lsu (shared / global / local memory), cbu (branches,
 convergence barriers), uniform (U* datapath)."""
 import collections
@@ -42,9 +45,20 @@ def loop_of(so, pat):
     return [(a, t) for a, t in ins if start <= a <= end]
 
 
+def option(name, default=None):
+    return sys.argv[sys.argv.index(name) + 1] if name in sys.argv else default
+
+
 def main():
     so, pat = sys.argv[1], sys.argv[2]
     loop = loop_of(so, pat)
+    excluded = []
+    for r in filter(None, option("--exclude", "").split(",")):
+        lo, hi = (int(x, 16) for x in r.split("-"))
+        excluded.append((lo, hi))
+    full = len(loop)
+    loop = [(a, t) for a, t in loop if not any(lo <= a <= hi for lo, hi in excluded)]
+    steps = int(option("--steps", "1"))
     mix, ops = collections.Counter(), collections.Counter()
     for _, t in loop:
         op = re.sub(r"^@!?U?P\d+\s+", "", t).split()[0].split(".")[0]
@@ -52,10 +66,13 @@ def main():
         mix[pipe] += 1
         ops[(pipe, op)] += 1
     n = len(loop)
-    print(f"{pat}: loop 0x{loop[0][0]:x}..0x{loop[-1][0]:x}, {n} instructions")
+    print(f"{pat}: loop 0x{loop[0][0]:x}..0x{loop[-1][0]:x}, {n} instructions"
+          + (f" ({full - n} in {len(excluded)} excluded ranges left out)" if excluded else ""))
     for pipe, c in mix.most_common():
         detail = ", ".join(f"{op} {k}" for (p, op), k in sorted(ops.items(), key=lambda x: -x[1]) if p == pipe)
-        print(f"  {pipe:8s} {c:4d} ({100 * c / n:4.1f} %)  {detail}")
+        print(f"  {pipe:8s} {c:4d} ({100 * c / n:4.1f} %)" + (f"  {c / steps:6.1f} per step" if steps > 1 else "") + f"  {detail}")
+    if steps > 1:
+        print(f"  issued   {n:4d}            {n / steps:6.1f} per step")
     if "--list" in sys.argv:
         for a, t in loop:
             print(f"    {a:05x}  {t}")
