@@ -511,6 +511,10 @@ struct Sim {
     using recorded_queue_type = objectqueue;    // ... a queue whose length history will be switched on
     using buffer_type = buffer;
     using recorded_buffer_type = buffer;
+    using resourcepool_type = resourcepool;
+    using recorded_resourcepool_type = resourcepool;
+    using resource_type = resource;
+    using recorded_resource_type = resource;
     Sfc64          rng;
     const ZigHot  *hot;
     double         now;

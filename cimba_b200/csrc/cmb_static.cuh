@@ -9,13 +9,15 @@
 //   * process records, guards (a bit and a sequence number per process) and the model struct stay in registers: process ids
 //     are compile-time constants after inlining, nothing takes an address;
 //   * a queue is a ring with its oldest 32 entries in shared memory and the rest in an HBM ring (StampRing, engine.cuh); a
-//     cmb_buffer is two counters; either can keep its time-weighted history (S::recorded_queue_type, S::recorded_buffer_type);
+//     cmb_buffer is two counters; a cmb_resourcepool is two counters and a holding per process, a cmb_resource its holder;
+//     each can keep its time-weighted history (S::recorded_queue_type, ..._buffer_type, ..._resourcepool_type, ..._resource_type);
 //   * blocking calls are commands carried out by the dispatcher where the warp is together, and the ziggurat's slow path
 //     is taken by parked lanes in batches - as in the fused kernels (queue_model.cuh, whose shape this generalises); a hold
 //     of any distribution can be drawn there too (CMB_PROCESS_HOLD_SAMPLED: rectangles first, rewind + park + batch otherwise).
-// What the tier does NOT have - process creation beyond NPROC, priorities other than 0, timers, interrupts, a queue that
-// outgrows window + ring - is not an error: the trial is flagged and the launch re-runs it on the general engine from the SAME
-// model template (launch_static_model below), so the answer is the reference's either way.
+// What the tier does NOT have - process creation beyond NPROC, priorities other than 0, timers, interrupts, pre-emption, a
+// process that exits or is stopped while it holds from a pool or a resource, a queue that outgrows window + ring - is not an
+// error: the trial is flagged and the launch re-runs it on the general engine from the SAME model template
+// (launch_static_model below), so the answer is the reference's either way.
 //
 // A model is `template <class S> struct M` with S = cmb::Sim or cmb::StaticSim<...>, its queues declared as
 // `typename S::queue_type`, exported with CMB_EXPORT_STATIC_MODEL(M, NPROC, NQUEUE, "name") (or ..._EVENTS(M, NPROC, NQUEUE,
@@ -149,6 +151,23 @@ struct static_buffer : static_history<RECORD> {
     uint64_t level, capacity;
 };
 
+// struct cmb_resourcepool for a fixed set of processes (src/cmb_resourcepool.c): the holders' records are a bit and an amount
+// per process, in registers like the rest; the history, when kept, is of in_use
+template <int NPROC, bool RECORD = false>
+struct static_resourcepool : static_history<RECORD> {
+    static_guard<NPROC> guard;
+    uint64_t capacity, in_use;
+    uint32_t holding;           // bit i: process i has a holder record (cmb_resourcepool_held_by_process finds it)
+    uint64_t held[NPROC];       // ... and the amount it holds
+};
+
+// struct cmb_resource, the binary semaphore (src/cmb_resource.c); the history, when kept, is 1 while held, 0 while free
+template <int NPROC, bool RECORD = false>
+struct static_resource : static_history<RECORD> {
+    static_guard<NPROC> guard;
+    uint32_t holder;            // process index, NIL = free
+};
+
 // NEVENT: how many events of its own (cmb_event_schedule) a model may have pending at once; with any, the event list also
 // orders by priority
 template <int NPROC, int NQUEUE, int NEVENT = 0>
@@ -157,8 +176,15 @@ struct StaticSim {
     using recorded_queue_type = static_objectqueue<NPROC, true>;
     using buffer_type = static_buffer<NPROC, false>;
     using recorded_buffer_type = static_buffer<NPROC, true>;
+    using resourcepool_type = static_resourcepool<NPROC, false>;
+    using recorded_resourcepool_type = static_resourcepool<NPROC, true>;
+    using resource_type = static_resource<NPROC, false>;
+    using recorded_resource_type = static_resource<NPROC, true>;
     static constexpr int PROCESSES = NPROC;
     static constexpr int SLOTS = NPROC + NEVENT;
+    static_assert(NPROC >= 1 && NPROC <= 32, "a guard's wait list is a 32-bit mask of processes");
+    static constexpr uint32_t HOLD_BITS = NPROC <= 8 ? 4u : (NPROC <= 16 ? 2u : 1u);
+    static constexpr uint32_t HOLD_MAX = (1u << HOLD_BITS) - 1u;
     struct Proc {
         uint32_t pc, status, kind, ctx;
         double   f[2];
@@ -178,6 +204,10 @@ struct StaticSim {
     uint32_t       current_event;
     uint32_t       pops;
     uint32_t       nproc, nqueue, guard_seq;
+    // how many pools and resources each process holds from, HOLD_BITS per process.  The reference drops a process's
+    // holdings when it exits or is stopped (cmi_process_drop_resources, src/cmb_process.c:507-527); this tier does not, and
+    // flags the trial instead.  One word, in what would otherwise be padding: a model that holds nothing keeps its layout.
+    uint32_t       holds;
     Proc           proc[NPROC];
     StaticFel<NPROC + NEVENT, (NEVENT > 0)> fel;
     UserEvent      uev[NEVENT > 0 ? NEVENT : 1];
@@ -203,6 +233,7 @@ struct StaticSim {
         current_event = 0u;
         pops = 0u;
         nproc = nqueue = guard_seq = 0u;
+        holds = 0u;
         fel.clear();
         cmd = CMD_NONE;
         cmd_sample = 0u;
@@ -223,6 +254,22 @@ struct StaticSim {
             proc[i].u[0] = proc[i].u[1] = 0u;
             proc[i].fr[0] = proc[i].fr[1] = proc[i].fr[2] = 0u;
             proc[i].exit_value = 0;
+        }
+    }
+
+    CMB_FN uint32_t holds_of(uint32_t pid) const { return (holds >> (pid * HOLD_BITS)) & HOLD_MAX; }
+
+    // process pid began (+1) or ceased (-1) to hold from a pool or a resource.  More holdings at once than HOLD_BITS count:
+    // the trial goes to the general engine.
+    CMB_FN void holds_add(uint32_t pid, int32_t d)
+    {
+        const uint32_t c = holds_of(pid);
+        if (d > 0) {
+            if (c == HOLD_MAX) status |= TRIAL_ERR_PROC_OVERFLOW;
+            else holds += 1u << (pid * HOLD_BITS);
+        }
+        else if (c > 0u) {
+            holds -= 1u << (pid * HOLD_BITS);
         }
     }
 
@@ -275,6 +322,7 @@ struct StaticSim {
     CMB_FN void process_start(uint32_t pid)             // src/cmb_process.c:127-135
     {
         if (!fel.schedule((int)pid, ACT_START, now)) status |= TRIAL_ERR_FEL_OVERFLOW;
+        if (holds_of(pid) != 0u) status |= TRIAL_ERR_PROC_OVERFLOW;    // restarted after it ended holding: see static_trial_end
     }
 
     CMB_FN int64_t hold_end(uint32_t, int64_t sig) { return sig; }          // nobody interrupts here
@@ -519,8 +567,202 @@ CMB_FN bool buffer_put_step(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &, stat
     return done;
 }
 
+// ------------------------------------------------------------------------------------------------ resourcepool
+// as cmb_device.cuh's functions of the same names (src/cmb_resourcepool.c), the holders' records in registers.  Every waiter
+// wants units (DEMAND_POOL_AVAILABLE), so a signal's demand is `capacity - in_use > 0`.
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void resourcepool_initialize(StaticSim<NPROC, NQUEUE, NEVENT> &, static_resourcepool<NPROC, RECORD> &rp, uint64_t capacity)
+{
+    rp.guard.waiting = 0u;
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) {
+        rp.guard.seq[i] = 0u;
+        rp.held[i] = 0u;
+    }
+    rp.capacity = capacity;
+    rp.in_use = 0u;
+    rp.holding = 0u;
+    if constexpr (RECORD) rp.recording = 0u;
+}
+
+template <int NPROC, int NQUEUE, int NEVENT>
+CMB_FN void resourcepool_recording_start(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resourcepool<NPROC, true> &rp)
+{
+    rp.recording = 1u;
+    rp.history.start();
+    rp.history.sample((double)rp.in_use, sim.now);
+}
+
+template <int NPROC, int NQUEUE, int NEVENT>
+CMB_FN void resourcepool_recording_stop(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resourcepool<NPROC, true> &rp)
+{
+    if (rp.recording) rp.history.sample((double)rp.in_use, sim.now);
+    rp.recording = 0u;
+}
+
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void pool_sample(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resourcepool<NPROC, RECORD> &rp)
+{
+    if constexpr (RECORD) {
+        if (rp.recording) rp.history.sample((double)rp.in_use, sim.now);
+    }
+}
+
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN uint64_t resourcepool_held_by_process(StaticSim<NPROC, NQUEUE, NEVENT> &, static_resourcepool<NPROC, RECORD> &rp, uint32_t pid)
+{
+    uint64_t h = 0u;
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) {
+        if ((uint32_t)i == pid) h = rp.held[i];
+    }
+    return h;
+}
+
+// update_record (src/cmb_resourcepool.c:324-355): the caller's record grows by `amount`, made if it had none
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void pool_update_record(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resourcepool<NPROC, RECORD> &rp, uint32_t pid, uint64_t amount)
+{
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) {
+        if ((uint32_t)i == pid) {
+            if (((rp.holding >> i) & 1u) == 0u) {
+                rp.holding |= 1u << i;
+                sim.holds_add(pid, 1);
+            }
+            rp.held[i] += amount;
+        }
+    }
+}
+
+// cmi_pool_acquire_inner up to its wait (:362-497): true = satisfied, false = the caller waits at the guard for the rest.
+// fr[1] = the remaining claim.  A grab that leaves the claim unmet keeps what it took (the greedy partial grab).
+// cmb_resourcepool_preempt may interrupt a holder, which this tier cannot: the trial goes to the general engine.
+template <class Model, int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN bool pool_acquire_step(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &, static_resourcepool<NPROC, RECORD> &rp, uint32_t pid,
+                              bool preempt)
+{
+    if (preempt) sim.status |= TRIAL_ERR_PROC_OVERFLOW;
+    uint64_t rem = 0u;
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) {
+        if ((uint32_t)i == pid) rem = sim.proc[i].fr[1];
+    }
+    const uint64_t available = rp.capacity - rp.in_use;
+    if (available >= rem) {
+        rp.in_use += rem;
+        pool_sample(sim, rp);
+        pool_update_record(sim, rp, pid, rem);
+        sim.guard_signal(rp.guard, rp.capacity - rp.in_use > 0u);
+        return true;
+    }
+    if (available > 0u) {
+        rp.in_use += available;
+        pool_sample(sim, rp);
+        rem -= available;
+        pool_update_record(sim, rp, pid, available);
+    }
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) {
+        if ((uint32_t)i == pid) sim.proc[i].fr[1] = rem;
+    }
+    return false;
+}
+
+// the tail of cmi_pool_acquire_inner after an unsuccessful wait (:499-531).  Only an interrupt, a timer or a pre-emption ends
+// a wait unsuccessfully, and none of them exists on this tier; should one ever get here, the general engine answers.
+template <class Model, int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void pool_acquire_rollback(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &, static_resourcepool<NPROC, RECORD> &, uint32_t, int64_t)
+{
+    sim.status |= TRIAL_ERR_PROC_OVERFLOW;
+}
+
+// cmb_resourcepool_release, :561-605
+template <class Model, int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void resourcepool_release(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &, static_resourcepool<NPROC, RECORD> &rp, uint32_t pid,
+                                 uint64_t amount)
+{
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) {
+        if ((uint32_t)i == pid && ((rp.holding >> i) & 1u) != 0u) {
+            if (rp.held[i] == amount) {
+                rp.holding &= ~(1u << i);
+                sim.holds_add(pid, -1);
+                rp.held[i] = 0u;
+            }
+            else {
+                rp.held[i] -= amount;
+            }
+        }
+    }
+    rp.in_use -= amount;
+    pool_sample(sim, rp);
+    sim.guard_signal(rp.guard, rp.capacity - rp.in_use > 0u);
+}
+
+// ------------------------------------------------------------------------------------------------ resource
+// as cmb_device.cuh's (src/cmb_resource.c); every waiter wants it free (DEMAND_RESOURCE_FREE)
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void resource_initialize(StaticSim<NPROC, NQUEUE, NEVENT> &, static_resource<NPROC, RECORD> &r)
+{
+    r.guard.waiting = 0u;
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) r.guard.seq[i] = 0u;
+    r.holder = NIL;
+    if constexpr (RECORD) r.recording = 0u;
+}
+
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void resource_sample(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resource<NPROC, RECORD> &r)       // record_sample
+{
+    if constexpr (RECORD) {
+        if (r.recording) r.history.sample(r.holder != NIL ? 1.0 : 0.0, sim.now);
+    }
+}
+
+template <int NPROC, int NQUEUE, int NEVENT>
+CMB_FN void resource_recording_start(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resource<NPROC, true> &r)
+{
+    r.recording = 1u;
+    r.history.start();
+    r.history.sample(r.holder != NIL ? 1.0 : 0.0, sim.now);
+}
+
+template <int NPROC, int NQUEUE, int NEVENT>
+CMB_FN void resource_recording_stop(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resource<NPROC, true> &r)
+{
+    resource_sample(sim, r);
+    r.recording = 0u;
+}
+
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void resource_grab(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resource<NPROC, RECORD> &r, uint32_t pid)     // :182-189
+{
+    r.holder = pid;
+    sim.holds_add(pid, 1);
+}
+
+template <class Model, int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN void resource_release(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &, static_resource<NPROC, RECORD> &r, uint32_t pid)  // :234-250
+{
+    if (r.holder == pid) sim.holds_add(pid, -1);
+    r.holder = NIL;
+    resource_sample(sim, r);
+    sim.guard_signal(r.guard, true);
+}
+
+// cmb_resource_preempt evicts a holder of equal or lower priority (:270-320), which takes an interrupt: the general engine's.
+// false = go on as cmb_resource_acquire (the trial is void by then, but runs to its end like any flagged trial).
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD>
+CMB_FN bool resource_preempt_step(StaticSim<NPROC, NQUEUE, NEVENT> &sim, static_resource<NPROC, RECORD> &, uint32_t)
+{
+    sim.status |= TRIAL_ERR_PROC_OVERFLOW;
+    return false;
+}
+
 // cmb_process_stop (src/cmb_process.c:698-723) as far as this tier can need it: the process's pending event goes, it is
-// FINISHED; an entry it may have in a guard stays (SURVEY.md quirk 2) and will swallow one signal
+// FINISHED; an entry it may have in a guard stays (SURVEY.md quirk 2) and will swallow one signal.  A process stopped while
+// it holds from a pool or a resource would drop its holdings: static_trial_end flags that.
 template <class Model, int NPROC, int NQUEUE, int NEVENT>
 CMB_FN void process_stop(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &, uint32_t pid, int64_t value)
 {
@@ -619,6 +861,21 @@ CMB_FN bool static_step(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &m, int &wh
     return true;
 }
 
+// The reference drops the holdings of a process that exits or is stopped (cmi_process_drop_resources, src/cmb_process.c:
+// 507-527: units back to the pool, the resource freed, their guards signalled); this tier does not.  Only a process itself
+// gives back what it holds, so one that ended holding still does when the trial ends - or when it is started again
+// (process_start).  Either way the trial goes to the general engine.  Checked here, once per trial, rather than at every exit:
+// a model that holds nothing keeps its code.
+template <int NPROC, int NQUEUE, int NEVENT>
+CMB_FN void static_trial_end(StaticSim<NPROC, NQUEUE, NEVENT> &sim)
+{
+    if (sim.holds == 0u) return;
+#pragma unroll
+    for (int i = 0; i < NPROC; i++) {
+        if (sim.proc[i].status == PROC_FINISHED && sim.holds_of((uint32_t)i) != 0u) sim.status |= TRIAL_ERR_PROC_OVERFLOW;
+    }
+}
+
 // the blocking call the body ended on, except the holds whose duration the caller draws (exponential, sampled)
 template <int NPROC, int NQUEUE, int NEVENT>
 CMB_FN void static_finish_command(StaticSim<NPROC, NQUEUE, NEVENT> &sim, int who, uint32_t cmd)
@@ -681,6 +938,7 @@ inline void static_run_trial_host(StaticSim<NPROC, NQUEUE, NEVENT> &sim, Model &
             static_finish_command(sim, who, cmd);
         }
     }
+    static_trial_end(sim);
     m.finish(sim, out);
 }
 #else
@@ -772,6 +1030,7 @@ static_trial_kernel(const StaticArgs sa)
         if (alive && !parked) {
             if (!static_step(sim, m, who)) {
                 alive = false;                          // cmb_event_queue_execute returns
+                static_trial_end(sim);
                 m.finish(sim, out);
                 if (a.events)    a.events[trial] = sim.pops;
                 if (a.objects)   a.objects[trial] = out.objects;
