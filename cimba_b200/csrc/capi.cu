@@ -83,67 +83,13 @@ int cuda_fail(cudaError_t e, const char *where)
         if (e_ != cudaSuccess) return cuda_fail(e_, #expr);        \
     } while (0)
 
-constexpr uint32_t QUEUE_SPILL_CAP = 512u;     // default: doubles per trial behind the 32-entry window
-
-// job.queue_spill_cap: 0 = default, else a power of two up to 2^26; 0xffffffff = invalid
-uint32_t spill_cap_of(const cimba_b200_device_job *job)
-{
-    const uint32_t c = job->queue_spill_cap;
-    if (c == 0u) return QUEUE_SPILL_CAP;
-    if ((c & (c - 1u)) != 0u || c > (1u << 26)) return 0xffffffffu;
-    return c;
-}
-
-// ---- the general engine behind the fixed-capacity fast kernels
-// A trial the fast M/M/1, G/G/1 or M/M/c kernel had to flag (its queue outgrew window + ring, its event list or wait list
-// their fixed tables) is re-run inside the same launch by the general engine, whose containers grow: the reference's
-// queue is CMB_UNLIMITED and so is the drop-in.  The repair kernel is enqueued unconditionally behind the fast one and
-// looks at the status words; with nothing flagged it costs one pass over them.
-constexpr uint32_t REPAIR_BITS = CIMBA_B200_TRIAL_QUEUE_OVERFLOW | CIMBA_B200_TRIAL_FEL_OVERFLOW |
-                                 CIMBA_B200_TRIAL_GUARD_OVERFLOW | CIMBA_B200_TRIAL_PROC_OVERFLOW;
-
+// growth arena of the repair pass behind the fixed-capacity kernels of the library (M/M/1, G/G/1, M/M/c, models 3-6, 8, 11-14)
 uint64_t repair_arena_bytes(const cimba_b200_device_job *job)
 {
     uint64_t b = job->num_trials * 32768ull;
     if (b < (64ull << 20)) b = 64ull << 20;
     if (b > (4ull << 30)) b = 4ull << 30;
     return cmb::ARENA_HEADER + b;
-}
-
-uint64_t align256(uint64_t v) { return (v + 255u) & ~(uint64_t)255u; }
-
-bool mmc_goes_general(const cimba_b200_device_job *job)
-{
-    return job->model == CIMBA_B200_MODEL_MMC && (job->variant == CIMBA_B200_VARIANT_GENERAL || job->servers > 14);
-}
-
-bool fast_goes_general(const cimba_b200_device_job *job)
-{
-    return (job->model == CIMBA_B200_MODEL_MM1 || job->model == CIMBA_B200_MODEL_GG1 || job->model == CIMBA_B200_MODEL_MM1_RECORDED) &&
-           job->variant == CIMBA_B200_VARIANT_GENERAL;
-}
-
-// the tutorial's trial runs on the static tier (two processes, a buffer, three events of its own) unless the general engine is asked for
-bool tutorial1_goes_static(const cimba_b200_device_job *job)
-{
-    return job->model == CIMBA_B200_MODEL_TUTORIAL1 && job->variant != CIMBA_B200_VARIANT_GENERAL;
-}
-
-bool goes_static(const cimba_b200_device_job *job)
-{
-    if (tutorial1_goes_static(job)) return true;
-    return (job->model == CIMBA_B200_MODEL_MM1 || job->model == CIMBA_B200_MODEL_GG1 || job->model == CIMBA_B200_MODEL_MM1_RECORDED) &&
-           job->variant == CIMBA_B200_VARIANT_STATIC;
-}
-
-bool hold_goes_general(const cimba_b200_device_job *job)
-{
-    return job->model == CIMBA_B200_MODEL_HOLD && job->variant == CIMBA_B200_VARIANT_GENERAL;
-}
-
-bool harbor_goes_general(const cimba_b200_device_job *job)
-{
-    return job->model == CIMBA_B200_MODEL_HARBOR && job->variant == CIMBA_B200_VARIANT_GENERAL;
 }
 
 // models loaded with cimba_b200_model_load
@@ -163,45 +109,6 @@ const UserModel *user_model(int id)
     return (k >= 0 && (size_t)k < g_user_models.size()) ? &g_user_models[(size_t)k] : nullptr;
 }
 
-template <class Model>
-int launch_general(const cimba_b200_device_job *job, unsigned char *arena, uint64_t bytes, uint32_t only_flagged, cudaStream_t st,
-                   const char *what)
-{
-    const int e = cmb::launch_model<Model>(*job, arena, bytes, only_flagged, st);
-    g_launches++;
-    return e == 0 ? CIMBA_B200_OK : cuda_fail((cudaError_t)e, what);
-}
-
-// the reference's own test worlds (models 3-6, 8, 11-14): like M/M/1, G/G/1 and M/M/c they have a fixed-capacity kernel
-// (csrc/general.cuh, faster than the engine) behind which the general engine re-runs whatever that
-// kernel flags; a capacity its tables cannot hold, or CIMBA_B200_VARIANT_GENERAL, goes to the engine directly
-bool coverage_goes_general(const cimba_b200_device_job *job);
-
-template <template <class> class F, class... A>
-auto for_coverage_model(int model, A &&...a)
-{
-    switch (model) {
-    case CIMBA_B200_MODEL_GUARDED:           return F<models::Guarded<false, false>>::call(a...);
-    case CIMBA_B200_MODEL_GUARDED_RECORDED:  return F<models::Guarded<false, true>>::call(a...);
-    case CIMBA_B200_MODEL_PRIOQ_RECORDED:    return F<models::Guarded<true, true>>::call(a...);
-    case CIMBA_B200_MODEL_PREEMPT:           return F<models::PoolFight>::call(a...);
-    case CIMBA_B200_MODEL_BUFFER:            return F<models::Workshop<false>>::call(a...);
-    case CIMBA_B200_MODEL_BUFFER_RECORDED:   return F<models::Workshop<true>>::call(a...);
-    case CIMBA_B200_MODEL_PRIOQ:             return F<models::QueueAndTide>::call(a...);
-    case CIMBA_B200_MODEL_TIMERS:            return F<models::FrontDesk>::call(a...);
-    default:                                 return F<models::Tool>::call(a...);       // CIMBA_B200_MODEL_RESOURCE_RECORDED
-    }
-}
-
-template <class Model>
-struct WorkspaceOf {
-    static uint64_t call(const cimba_b200_device_job *job) { return cmb::workspace_bytes_for<Model>(*job); }
-};
-
-bool is_queue_model(int m)
-{
-    return m == CIMBA_B200_MODEL_MM1 || m == CIMBA_B200_MODEL_GG1 || m == CIMBA_B200_MODEL_MM1_RECORDED;
-}
 #ifndef HOLD_DEFAULT_LANES
 #define HOLD_DEFAULT_LANES 32      // lanes per trial of the default hold kernel (H100, 4096 trials x 1000 workers: 32 -> 304 ms, 16 -> 415, 8 -> 745)
 #endif
@@ -213,32 +120,6 @@ uint64_t deep_row_entries(int workers)
     const uint64_t below = count > 33u ? count - 33u : 0u;
     return ((below + 31u) / 32u) * 32u + 32u;
 }
-
-bool is_general_model(int m)
-{
-    return m == CIMBA_B200_MODEL_GUARDED || m == CIMBA_B200_MODEL_PREEMPT || m == CIMBA_B200_MODEL_BUFFER ||
-           m == CIMBA_B200_MODEL_PRIOQ || m == CIMBA_B200_MODEL_TIMERS || m == CIMBA_B200_MODEL_GUARDED_RECORDED ||
-           m == CIMBA_B200_MODEL_BUFFER_RECORDED || m == CIMBA_B200_MODEL_PRIOQ_RECORDED ||
-           m == CIMBA_B200_MODEL_RESOURCE_RECORDED;
-}
-
-bool coverage_goes_general(const cimba_b200_device_job *job)
-{
-    if (!is_general_model(job->model)) return false;
-    if (job->variant == CIMBA_B200_VARIANT_GENERAL) return true;
-    const int m = job->model;
-    if (m == CIMBA_B200_MODEL_TIMERS || m == CIMBA_B200_MODEL_RESOURCE_RECORDED || m == CIMBA_B200_MODEL_PREEMPT ||
-        m == CIMBA_B200_MODEL_BUFFER || m == CIMBA_B200_MODEL_BUFFER_RECORDED) return false;      // no table sized by `servers`
-    return job->servers > ((m == CIMBA_B200_MODEL_PRIOQ || m == CIMBA_B200_MODEL_PRIOQ_RECORDED) ? 15 : 16);
-}
-
-template <class Model>
-struct LaunchOf {
-    static int call(const cimba_b200_device_job *job, unsigned char *arena, uint64_t bytes, uint32_t only_flagged, cudaStream_t st)
-    {
-        return launch_general<Model>(job, arena, bytes, only_flagged, st, only_flagged ? "repair pass" : "trial_kernel launch");
-    }
-};
 
 // ---------------------------------------------------------------- RNG KAT kernel
 __global__ void rng_draws_kernel(uint64_t seed, int kind, double p0, double p1, uint64_t n, double *out)
@@ -370,18 +251,419 @@ AwacsOrbit awacs_orbit()
     return o;
 }
 
-template <int MODEL>
-int launch_queue(const QueueArgs &qa, bool trace, dim3 grid, cudaStream_t st)
+// ---------------------------------------------------------------- routes
+// A route is the code that serves a job: what workspace it needs and how it launches.  route() picks it; its launch
+// runs after cimba_b200_launch's common checks and makes the checks of its own.
+struct Route {
+    uint64_t (*workspace)(const cimba_b200_device_job *);
+    int (*launch)(const cimba_b200_device_job *, cudaStream_t);
+};
+
+int mapping_of(const cimba_b200_device_job *job) { return job->mapping == 0 ? CIMBA_B200_MAP_LANE : job->mapping; }
+
+int check_workspace(const cimba_b200_device_job *job)
 {
-    if (trace) {
-        queue_kernel<MODEL, true><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
+    if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
+        return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
+    return CIMBA_B200_OK;
+}
+
+// a launch made by cmb_launch.cuh (a cudaError_t as int) that started `launches` kernels
+int counted(int e, const char *what, int launches = 1)
+{
+    g_launches += launches;
+    return e == 0 ? CIMBA_B200_OK : cuda_fail((cudaError_t)e, what);
+}
+
+// a kernel of the library, in its TRACE instantiation when the job records pops
+template <class Args>
+int launch_kernel(const cimba_b200_device_job *job, void (*plain)(Args), void (*traced)(Args), dim3 grid, unsigned block,
+                  size_t smem, cudaStream_t st, const Args &a, const char *what)
+{
+    void (*const kernel)(Args) = job->trace_cap > 0u ? traced : plain;
+    kernel<<<grid, block, smem, st>>>(a);
+    g_launches++;
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? CIMBA_B200_OK : cuda_fail(e, what);
+}
+
+// after a fixed-capacity kernel (result e): the general engine re-runs what it flagged, in the arena behind its rings
+template <class Model>
+int then_repair(int e, const cimba_b200_device_job *job, uint64_t rings_bytes, cudaStream_t st, const char *what)
+{
+    if (e != CIMBA_B200_OK || job->status == nullptr) return e;       // nobody could see a flag: nothing to repair by
+    return counted(cmb::launch_repair<Model>(*job, rings_bytes, repair_arena_bytes(job), st), what);
+}
+
+// persistent CTAs: as many as are resident at once (`fallback` per SM if the occupancy query fails), at most `wanted`
+int resident_grid(const void *fn, int block, size_t smem, int fallback, uint64_t wanted, unsigned *grid)
+{
+    int dev = 0, sms = 132, per_sm = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, block, smem);
+    if (oe != cudaSuccess || per_sm < 1) per_sm = fallback;
+    const uint64_t resident = (uint64_t)sms * (uint64_t)per_sm;
+    *grid = (unsigned)(wanted < resident ? wanted : resident);
+    return CIMBA_B200_OK;
+}
+
+// ---- the general engine over every trial (growable event list, wait lists and queues)
+template <class Model>
+uint64_t engine_workspace(const cimba_b200_device_job *job) { return cmb::workspace_bytes_for<Model>(*job); }
+
+// servers_msg = NULL: the model has no capacity to check
+int engine_checks(const cimba_b200_device_job *job, const char *servers_msg)
+{
+    if (mapping_of(job) != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "the general engine runs one trial per lane (CIMBA_B200_MAP_LANE)");
+    if (servers_msg != nullptr && job->servers < 1) return fail(CIMBA_B200_EINVAL, servers_msg);
+    return check_workspace(job);
+}
+
+template <class Model>
+int launch_engine(const cimba_b200_device_job *job, cudaStream_t st, const char *what)
+{
+    return counted(cmb::launch_model<Model>(*job, (unsigned char *)job->workspace, job->workspace_bytes, 0u, st), what);
+}
+
+template <class Model> const char *const ENGINE_WHAT = nullptr;
+template <> const char *const ENGINE_WHAT<models::MM1> = "trial_kernel<MM1> launch";
+template <> const char *const ENGINE_WHAT<models::GG1> = "trial_kernel<GG1> launch";
+template <> const char *const ENGINE_WHAT<models::MM1Recorded> = "trial_kernel<MM1Recorded> launch";
+template <> const char *const ENGINE_WHAT<models::MMC> = "trial_kernel<MMC> launch";
+template <> const char *const ENGINE_WHAT<models::HoldGeneral> = "trial_kernel<HoldGeneral> launch";
+template <> const char *const ENGINE_WHAT<models::Renege> = "trial_kernel<Renege> launch";
+template <> const char *const ENGINE_WHAT<models::Cheese> = "trial_kernel<Cheese> launch";
+template <> const char *const ENGINE_WHAT<models::Tutorial1> = "trial_kernel<Tutorial1> launch";
+template <> const char *const ENGINE_WHAT<models::Park> = "trial_kernel<Park> launch";
+template <> const char *const ENGINE_WHAT<models::Tutorial2> = "trial_kernel<Tutorial2> launch";
+
+template <class Model>
+int engine_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (const int e = engine_checks(job, "servers must be >= 1")) return e;
+    return launch_engine<Model>(job, st, ENGINE_WHAT<Model>);
+}
+
+template <class Model>
+constexpr Route ENGINE{engine_workspace<Model>, engine_launch<Model>};
+
+int harbor_engine_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (const int e = engine_checks(job, "servers must be >= 1")) return e;
+    if (job->servers < 3) return fail(CIMBA_B200_EINVAL, "tugs (servers) must be >= 3 for CIMBA_B200_MODEL_HARBOR (a large ship needs 3)");
+    return launch_engine<models::HarborGeneral>(job, st, "trial_kernel<HarborGeneral> launch");
+}
+
+// ---- the static tier (cmb_static.cuh): ModelT<StaticSim<NPROC, NQUEUE>> first, ModelT<Sim> for what it flags
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
+uint64_t static_workspace(const cimba_b200_device_job *job) { return cmb::workspace_bytes_static<ModelT, NPROC, NQUEUE, NEVENT>(*job); }
+
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
+int static_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (mapping_of(job) != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "the static tier runs one trial per lane (CIMBA_B200_MAP_LANE)");
+    if (const int e = check_workspace(job)) return e;
+    return counted(cmb::launch_static_model<ModelT, NPROC, NQUEUE, NEVENT>(*job, st), "static_trial_kernel launch",
+                   job->status != nullptr ? 2 : 1);
+}
+
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
+constexpr Route STATIC{static_workspace<ModelT, NPROC, NQUEUE, NEVENT>, static_launch<ModelT, NPROC, NQUEUE, NEVENT>};
+
+// ---- the fused M/M/1, G/G/1 and M/M/c kernels: a queue window on chip, a ring per trial in HBM
+uint64_t queue_rings_bytes(const cimba_b200_device_job *job)
+{
+    const uint32_t cap = cmb::spill_cap(*job);
+    return job->num_trials * (uint64_t)(cap == 0u ? cmb::SPILL_CAP_DEFAULT : cap) * sizeof(double);
+}
+
+uint64_t queue_workspace(const cimba_b200_device_job *job) { return cmb::rings_then_arena(queue_rings_bytes(job), repair_arena_bytes(job)); }
+
+int queue_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (const int e = check_workspace(job)) return e;
+    const int mapping = mapping_of(job);
+    QueueArgs qa = cmb::job_args<QueueArgs>(*job);
+    qa.mapping = mapping;
+    qa.num_objects = job->num_objects;
+    qa.arr_mean = job->arr_mean;
+    qa.srv_mean = job->srv_mean;
+    qa.counters = job->counters;
+    qa.spill = (double *)job->workspace;
+    qa.spill_cap = cmb::spill_cap(*job);
+    qa.diag = (unsigned long long *)job->diag;
+    const uint64_t threads = job->num_trials * (uint64_t)mapping;
+    const uint64_t blocks = (threads + QUEUE_BLOCK - 1) / QUEUE_BLOCK;
+    if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
+    const dim3 grid((unsigned)blocks);
+    const uint64_t rings = queue_rings_bytes(job);
+    if (job->model == CIMBA_B200_MODEL_GG1) {
+        if (job->variant == 1) return launch_kernel(job, queue_kernel<1, false>, queue_kernel<1, true>, grid, QUEUE_BLOCK, 0, st, qa, "queue_kernel launch");
+        return then_repair<models::GG1>(launch_kernel(job, gg1_kernel<false>, gg1_kernel<true>, grid, QUEUE_BLOCK, 0, st, qa, "gg1_kernel launch"),
+                                        job, rings, st, "repair pass (G/G/1)");
+    }
+    if (job->model == CIMBA_B200_MODEL_MM1_RECORDED) {
+        if (job->counters == nullptr)
+            return fail(CIMBA_B200_EINVAL, "CIMBA_B200_MODEL_MM1_RECORDED writes its cmb_wtdsummary to counters[]");
+        const int e = launch_kernel(job, queue_kernel<0, false, true>, queue_kernel<0, true, true>, grid, QUEUE_BLOCK, 0, st, qa,
+                                    "queue_kernel (recorded) launch");
+        return then_repair<models::MM1Recorded>(e, job, rings, st, "repair pass (M/M/1 with its queue history)");
+    }
+    if (job->variant == 1) return launch_kernel(job, queue_kernel<0, false>, queue_kernel<0, true>, grid, QUEUE_BLOCK, 0, st, qa, "queue_kernel launch");
+    int e;
+    if (job->variant == 2) {                        // variates from producer warps (mm1_pc.cuh): an experiment, same answers
+        if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "variant 2 of MODEL_MM1 runs one trial per lane");
+        const dim3 pc_grid((unsigned)((job->num_trials + MM1_PC_CONSUMERS - 1) / MM1_PC_CONSUMERS));
+        e = launch_kernel(job, mm1_pc_kernel<false>, mm1_pc_kernel<true>, pc_grid, 2 * MM1_PC_CONSUMERS, 0, st, qa, "mm1_kernel launch");
     }
     else {
-        queue_kernel<MODEL, false><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
+        e = launch_kernel(job, mm1_kernel<false>, mm1_kernel<true>, grid, QUEUE_BLOCK, 0, st, qa, "mm1_kernel launch");
     }
-    g_launches++;
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? CIMBA_B200_OK : cuda_fail(e, "queue_kernel launch");
+    return then_repair<models::MM1>(e, job, rings, st, "repair pass (M/M/1)");
+}
+
+int mmc_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (job->servers < 1) return fail(CIMBA_B200_EINVAL, "servers must be >= 1 for CIMBA_B200_MODEL_MMC");
+    if (mapping_of(job) != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "MODEL_MMC supports CIMBA_B200_MAP_LANE only");
+    if (const int e = check_workspace(job)) return e;
+    PoolArgs pa = cmb::job_args<PoolArgs>(*job);
+    pa.servers = job->servers;
+    pa.num_objects = job->num_objects;
+    pa.arr_mean = job->arr_mean;
+    pa.srv_mean = job->srv_mean;
+    pa.spill = (double *)job->workspace;
+    pa.spill_cap = cmb::spill_cap(*job);
+    pa.diag = (unsigned long long *)job->diag;
+    const uint64_t blocks = (job->num_trials + POOL_BLOCK - 1) / POOL_BLOCK;
+    if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
+    const bool readable = job->variant == 1;        // the readable formulation, pool_model.cuh
+    const int e = launch_kernel(job, readable ? pool_kernel<false> : pool_fast_kernel<false>, readable ? pool_kernel<true> : pool_fast_kernel<true>,
+                                dim3((unsigned)blocks), POOL_BLOCK, 0, st, pa, "pool_kernel launch");
+    return then_repair<models::MMC>(e, job, queue_rings_bytes(job), st, "repair pass (M/M/c)");
+}
+
+// ---- the reference's own test worlds (models 3-6, 8, 11-14): a fixed-capacity kernel each (csrc/general.cuh, faster than
+// the engine) behind which the general engine re-runs whatever that kernel flags
+bool has_capacity(const cimba_b200_device_job *job)
+{
+    return job->model != CIMBA_B200_MODEL_TIMERS && job->model != CIMBA_B200_MODEL_RESOURCE_RECORDED;
+}
+
+template <bool TRACE>
+auto coverage_kernel(int m)
+{
+    return m == CIMBA_B200_MODEL_RESOURCE_RECORDED ? resource_kernel<TRACE>
+         : m == CIMBA_B200_MODEL_TIMERS ? timers_kernel<TRACE>
+         : m == CIMBA_B200_MODEL_PRIOQ ? prioq_kernel<TRACE>
+         : m == CIMBA_B200_MODEL_BUFFER || m == CIMBA_B200_MODEL_BUFFER_RECORDED ? buffer_kernel<TRACE>
+         : m == CIMBA_B200_MODEL_PREEMPT ? preempt_kernel<TRACE>
+                                         : guarded_kernel<TRACE>;
+}
+
+uint64_t coverage_workspace(const cimba_b200_device_job *job)
+{
+    return cmb::rings_then_arena(job->num_trials * (uint64_t)sizeof(GeneralState), repair_arena_bytes(job));
+}
+
+template <class Model>
+int coverage_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    const int m = job->model;
+    if (has_capacity(job) && job->servers < 1) return fail(CIMBA_B200_EINVAL, "capacity (servers) must be >= 1");
+    if (mapping_of(job) != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "MODEL_GUARDED supports CIMBA_B200_MAP_LANE only");
+    if (const int e = check_workspace(job)) return e;
+    GuardedArgs ga = cmb::job_args<GuardedArgs>(*job);
+    ga.capacity = job->servers;
+    ga.duration = job->num_objects;
+    ga.put_mean = job->arr_mean;
+    ga.get_mean = job->srv_mean;
+    ga.counters = job->counters;
+    ga.state = (GeneralState *)job->workspace;
+    ga.record = (m == CIMBA_B200_MODEL_GUARDED_RECORDED || m == CIMBA_B200_MODEL_BUFFER_RECORDED || m == CIMBA_B200_MODEL_PRIOQ_RECORDED) ? 1u : 0u;
+    ga.use_pq = m == CIMBA_B200_MODEL_PRIOQ_RECORDED ? 1u : 0u;
+    const uint64_t blocks = (job->num_trials + GUARDED_BLOCK - 1) / GUARDED_BLOCK;
+    if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
+    const int e = launch_kernel(job, coverage_kernel<false>(m), coverage_kernel<true>(m), dim3((unsigned)blocks), GUARDED_BLOCK, 0, st, ga,
+                                "guarded_kernel launch");
+    return then_repair<Model>(e, job, job->num_trials * (uint64_t)sizeof(GeneralState), st, "repair pass");
+}
+
+template <class Model>
+int coverage_engine_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (const int e = engine_checks(job, has_capacity(job) ? "capacity (servers) must be >= 1" : nullptr)) return e;
+    return launch_engine<Model>(job, st, "trial_kernel launch");
+}
+
+// CIMBA_B200_VARIANT_GENERAL, or more servers than the kernel's tables hold (max_servers), goes to the engine directly
+template <class Model>
+const Route *coverage_route(const cimba_b200_device_job *job, int max_servers)
+{
+    static constexpr Route fast{coverage_workspace, coverage_launch<Model>};
+    static constexpr Route engine{engine_workspace<Model>, coverage_engine_launch<Model>};
+    return job->variant == CIMBA_B200_VARIANT_GENERAL || job->servers > max_servers ? &engine : &fast;
+}
+
+// ---- the harbor: up to 32 768 trials warp-per-trial with the state in shared memory, the rest lane-per-trial in HBM
+uint64_t harbor_workspace(const cimba_b200_device_job *job) { return job->num_trials * (uint64_t)sizeof(HarborState); }
+
+int harbor_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (job->servers < 3 || job->servers > 255)
+        return fail(CIMBA_B200_EINVAL, "tugs (servers) must be in 3..255 for CIMBA_B200_MODEL_HARBOR (a large ship needs 3)");
+    if (mapping_of(job) != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "MODEL_HARBOR supports CIMBA_B200_MAP_LANE only");
+    if (const int e = check_workspace(job)) return e;
+    HarborArgs ha = cmb::job_args<HarborArgs>(*job);
+    ha.tugs = job->servers;
+    ha.duration = job->num_objects;
+    ha.arr_mean = job->arr_mean;
+    ha.unload_small = job->srv_mean;
+    ha.counters = job->counters;
+    ha.state = job->workspace;
+    // variant 0: up to 32 768 trials run warp-per-trial with the state in shared memory, and whatever trial
+    // outgrew those tables is re-run by the lane-per-trial kernel with the large HBM-resident tables; more
+    // trials go lane-per-trial directly.  (H100, 400 W, 600 h per trial: warp-per-trial 44 / 154 / 299 ms
+    // at 4096 / 16 384 / 32 768 trials, lane-per-trial 151 / 200 / 406 ms.)
+    // variant 1 = warp-per-trial only (overflow -> status), variant 2 = lane-per-trial only.
+    const bool on_chip_first = job->variant == 1 ||
+                               (job->variant == 0 && job->num_trials <= 32768u && job->status != nullptr);
+    ha.repair = 0u;
+    if (on_chip_first) {
+        const size_t smem = (HARBOR_BLOCK_ON_CHIP / 32) * sizeof(HarborStateOnChip);
+        const void *fn = job->trace_cap > 0u ? (const void *)harbor_on_chip_kernel<true> : (const void *)harbor_on_chip_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const uint64_t per_block = HARBOR_BLOCK_ON_CHIP / 32;
+        unsigned nb = 0;
+        if (const int e = resident_grid(fn, HARBOR_BLOCK_ON_CHIP, smem, 4, (job->num_trials + per_block - 1) / per_block, &nb)) return e;
+        const int e = launch_kernel(job, harbor_on_chip_kernel<false>, harbor_on_chip_kernel<true>, dim3(nb), HARBOR_BLOCK_ON_CHIP, smem, st, ha,
+                                    "harbor_on_chip_kernel launch");
+        if (e != CIMBA_B200_OK || job->variant == 1) return e;
+        ha.repair = 1u;
+    }
+    const uint64_t blocks = (job->num_trials + GUARDED_BLOCK - 1) / GUARDED_BLOCK;
+    if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
+    return launch_kernel(job, harbor_kernel<false>, harbor_kernel<true>, dim3((unsigned)blocks), GUARDED_BLOCK, 0, st, ha, "harbor_kernel launch");
+}
+
+// ---- AWACS: one trial per warp over the terrain registered for the device
+uint64_t awacs_workspace(const cimba_b200_device_job *job) { return job->num_trials * (uint64_t)AWACS_STATE_BYTES; }
+
+int awacs_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (job->num_objects == 0u) return fail(CIMBA_B200_EINVAL, "MODEL_AWACS: num_objects = trial duration in seconds, > 0");
+    if (const int e = check_workspace(job)) return e;
+    int dev = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    AwacsArgs aa = cmb::job_args<AwacsArgs>(*job);
+    {
+        std::lock_guard<std::mutex> hold(g_terrain_mu);
+        if (dev < 0 || dev >= MAX_TERRAIN_DEVICES || !g_terrain_set[dev])
+            return fail(CIMBA_B200_EINVAL, "MODEL_AWACS: no terrain registered on this device; call cimba_b200_awacs_set_terrain()");
+        aa.ter = g_terrain[dev];
+    }
+    aa.orbit = awacs_orbit();
+    aa.t_end_s = (double)job->num_objects;
+    aa.state = (unsigned char *)job->workspace;
+    aa.counters = job->counters;
+    const uint64_t per_block = AWACS_BLOCK / 32;
+    const uint64_t blocks = (job->num_trials + per_block - 1) / per_block;
+    if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
+    return launch_kernel(job, awacs_kernel<false>, awacs_kernel<true>, dim3((unsigned)blocks), AWACS_BLOCK, 0, st, aa, "awacs_kernel launch");
+}
+
+// ---- the hold model: variant 1 keeps the whole list in shared memory (hold_model.cuh); the others keep levels >= 2 of
+// the 32-ary heap in HBM/L2 (hold_deep.cuh), with 32 (variant 2), 16 (3), 8 (4) or HOLD_DEFAULT_LANES (0) lanes per trial
+uint64_t hold_workspace(const cimba_b200_device_job *job)
+{
+    return job->variant != 1 ? job->num_trials * deep_row_entries(job->servers) * (uint64_t)sizeof(uint4) : 0u;
+}
+
+template <bool TRACE>
+auto deep_kernel(int lanes)
+{
+    return lanes == 32 ? hold_deep_kernel<TRACE> : lanes == 16 ? hold_group_kernel<16, TRACE> : hold_group_kernel<8, TRACE>;
+}
+
+int hold_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    const bool on_chip = job->variant == 1;
+    if (job->servers < 1 || (on_chip && job->servers > HOLD_CAP - 8) ||
+        (uint32_t)job->servers + 2u > DEEP_MAX_ENTRIES)
+        return fail(CIMBA_B200_EINVAL, "workers (servers) must be in 1..33822 for CIMBA_B200_MODEL_HOLD (1..1080 with variant 1)");
+    const bool trace = job->trace_cap > 0u;
+    HoldArgs ha = cmb::job_args<HoldArgs>(*job);
+    ha.workers = job->servers;
+    ha.duration = job->num_objects;
+    ha.mean = job->arr_mean;
+    ha.counters = job->counters;
+    unsigned blocks = 0;
+    if (!on_chip) {
+        if (const int e = check_workspace(job)) return e;
+        const int lanes = job->variant == 2 ? 32 : (job->variant == 4 ? 8 : (job->variant == 3 ? 16 : HOLD_DEFAULT_LANES));
+        const void *fn = trace ? (const void *)deep_kernel<true>(lanes) : (const void *)deep_kernel<false>(lanes);
+        const uint64_t trials_per_block = (uint64_t)(DEEP_BLOCK / 32) * (uint64_t)(32 / lanes);
+        if (const int e = resident_grid(fn, DEEP_BLOCK, 0, 8, (job->num_trials + trials_per_block - 1) / trials_per_block, &blocks)) return e;
+        DeepArgs da{};
+        da.h = ha;
+        da.rows = (uint4 *)job->workspace;
+        da.row_entries = deep_row_entries(job->servers);
+        return launch_kernel(job, deep_kernel<false>(lanes), deep_kernel<true>(lanes), dim3(blocks), DEEP_BLOCK, 0, st, da, "hold_deep_kernel launch");
+    }
+    // persistent one-warp CTAs: exactly as many as are resident at once (shared memory
+    // bounds it at ~12 per SM), so no CTA waits for another to retire
+    const void *fn = trace ? (const void *)hold_kernel<true> : (const void *)hold_kernel<false>;
+    if (const int e = resident_grid(fn, 32, HOLD_SMEM_BYTES, 8, job->num_trials, &blocks)) return e;
+    return launch_kernel(job, hold_kernel<false>, hold_kernel<true>, dim3(blocks), 32, HOLD_SMEM_BYTES, st, ha, "hold_kernel launch");
+}
+
+// ---- a model loaded with cimba_b200_model_load
+uint64_t user_workspace(const cimba_b200_device_job *job) { return user_model(job->model)->workspace_bytes(job); }
+
+int user_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (const int e = check_workspace(job)) return e;
+    const UserModel *um = user_model(job->model);
+    return counted(um->launch(job, st), um->name.c_str());
+}
+
+constexpr Route QUEUE{queue_workspace, queue_launch};
+constexpr Route MMC_FAST{queue_workspace, mmc_launch};
+constexpr Route HARBOR{harbor_workspace, harbor_launch};
+constexpr Route HARBOR_ENGINE{engine_workspace<models::HarborGeneral>, harbor_engine_launch};
+constexpr Route AWACS{awacs_workspace, awacs_launch};
+constexpr Route HOLD{hold_workspace, hold_launch};
+constexpr Route USER{user_workspace, user_launch};
+
+// The route that serves the job, nullptr for an unknown model
+const Route *route(const cimba_b200_device_job *job)
+{
+    const bool general = job->variant == CIMBA_B200_VARIANT_GENERAL, on_static = job->variant == CIMBA_B200_VARIANT_STATIC;
+    switch (job->model) {
+    case CIMBA_B200_MODEL_MM1:          return on_static ? &STATIC<models::MM1T, 2, 1> : general ? &ENGINE<models::MM1> : &QUEUE;
+    case CIMBA_B200_MODEL_GG1:          return on_static ? &STATIC<models::GG1T, 2, 1> : general ? &ENGINE<models::GG1> : &QUEUE;
+    case CIMBA_B200_MODEL_MM1_RECORDED: return on_static ? &STATIC<models::MM1RecordedT, 2, 1> : general ? &ENGINE<models::MM1Recorded> : &QUEUE;
+    case CIMBA_B200_MODEL_TUTORIAL1:    return general ? &ENGINE<models::Tutorial1> : &STATIC<models::Tutorial1T, 2, 0, 3>;
+    case CIMBA_B200_MODEL_MMC:          return general || job->servers > 14 ? &ENGINE<models::MMC> : &MMC_FAST;
+    case CIMBA_B200_MODEL_HOLD:         return general ? &ENGINE<models::HoldGeneral> : &HOLD;
+    case CIMBA_B200_MODEL_HARBOR:       return general ? &HARBOR_ENGINE : &HARBOR;
+    case CIMBA_B200_MODEL_AWACS:        return &AWACS;
+    case CIMBA_B200_MODEL_RENEGE:       return &ENGINE<models::Renege>;
+    case CIMBA_B200_MODEL_POOL_RECORDED: return &ENGINE<models::Cheese>;
+    case CIMBA_B200_MODEL_PARK:         return &ENGINE<models::Park>;
+    case CIMBA_B200_MODEL_TUTORIAL2:    return &ENGINE<models::Tutorial2>;
+    case CIMBA_B200_MODEL_GUARDED:            return coverage_route<models::Guarded<false, false>>(job, 16);
+    case CIMBA_B200_MODEL_GUARDED_RECORDED:   return coverage_route<models::Guarded<false, true>>(job, 16);
+    case CIMBA_B200_MODEL_PRIOQ_RECORDED:     return coverage_route<models::Guarded<true, true>>(job, 15);
+    case CIMBA_B200_MODEL_PRIOQ:              return coverage_route<models::QueueAndTide>(job, 15);
+    case CIMBA_B200_MODEL_PREEMPT:            return coverage_route<models::PoolFight>(job, INT32_MAX);   // no table sized by `servers`
+    case CIMBA_B200_MODEL_BUFFER:             return coverage_route<models::Workshop<false>>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_BUFFER_RECORDED:    return coverage_route<models::Workshop<true>>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_TIMERS:             return coverage_route<models::FrontDesk>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_RESOURCE_RECORDED:  return coverage_route<models::Tool>(job, INT32_MAX);
+    }
+    return job->model >= CIMBA_B200_MODEL_USER_BASE && user_model(job->model) != nullptr ? &USER : nullptr;
 }
 
 }  // namespace
@@ -405,52 +687,8 @@ int cimba_b200_device_count(void)
 
 uint64_t cimba_b200_workspace_bytes(const cimba_b200_device_job *job)
 {
-    if (job == nullptr) {
-        return 0u;
-    }
-    if (job->model >= CIMBA_B200_MODEL_USER_BASE) {
-        const UserModel *um = user_model(job->model);
-        return um ? um->workspace_bytes(job) : 0u;
-    }
-    if (job->model == CIMBA_B200_MODEL_RENEGE) return cmb::workspace_bytes_for<models::Renege>(*job);
-    if (job->model == CIMBA_B200_MODEL_POOL_RECORDED) return cmb::workspace_bytes_for<models::Cheese>(*job);
-    if (job->model == CIMBA_B200_MODEL_PARK) return cmb::workspace_bytes_for<models::Park>(*job);
-    if (job->model == CIMBA_B200_MODEL_TUTORIAL2) return cmb::workspace_bytes_for<models::Tutorial2>(*job);
-    if (job->model == CIMBA_B200_MODEL_TUTORIAL1 && !tutorial1_goes_static(job)) return cmb::workspace_bytes_for<models::Tutorial1>(*job);
-    if (coverage_goes_general(job)) return for_coverage_model<WorkspaceOf>(job->model, job);
-    if (mmc_goes_general(job)) return cmb::workspace_bytes_for<models::MMC>(*job);
-    if (hold_goes_general(job)) return cmb::workspace_bytes_for<models::HoldGeneral>(*job);
-    if (harbor_goes_general(job)) return cmb::workspace_bytes_for<models::HarborGeneral>(*job);
-    if (goes_static(job)) {
-        if (job->model == CIMBA_B200_MODEL_TUTORIAL1) return cmb::workspace_bytes_static<models::Tutorial1T, 2, 0, 3>(*job);
-        return job->model == CIMBA_B200_MODEL_MM1 ? cmb::workspace_bytes_static<models::MM1T, 2, 1>(*job)
-             : job->model == CIMBA_B200_MODEL_GG1 ? cmb::workspace_bytes_static<models::GG1T, 2, 1>(*job)
-                                                  : cmb::workspace_bytes_static<models::MM1RecordedT, 2, 1>(*job);
-    }
-    if (fast_goes_general(job)) {
-        return job->model == CIMBA_B200_MODEL_MM1 ? cmb::workspace_bytes_for<models::MM1>(*job)
-             : job->model == CIMBA_B200_MODEL_GG1 ? cmb::workspace_bytes_for<models::GG1>(*job)
-                                                  : cmb::workspace_bytes_for<models::MM1Recorded>(*job);
-    }
-    if (is_queue_model(job->model) || job->model == CIMBA_B200_MODEL_MMC) {
-        const uint32_t cap = spill_cap_of(job);
-        const uint64_t rings = job->num_trials * (uint64_t)(cap == 0xffffffffu ? QUEUE_SPILL_CAP : cap) * sizeof(double);
-        // the rings of the fast kernel, then the growth arena of its repair pass
-        return align256(rings) + repair_arena_bytes(job);
-    }
-    if (job->model == CIMBA_B200_MODEL_HARBOR) {
-        return job->num_trials * (uint64_t)sizeof(HarborState);
-    }
-    if (job->model == CIMBA_B200_MODEL_HOLD && job->variant != 1) {
-        return job->num_trials * deep_row_entries(job->servers) * (uint64_t)sizeof(uint4);
-    }
-    if (job->model == CIMBA_B200_MODEL_AWACS) {
-        return job->num_trials * (uint64_t)AWACS_STATE_BYTES;
-    }
-    if (is_general_model(job->model)) {
-        return align256(job->num_trials * (uint64_t)sizeof(GeneralState)) + repair_arena_bytes(job);
-    }
-    return 0u;
+    const Route *r = job != nullptr ? route(job) : nullptr;
+    return r != nullptr ? r->workspace(job) : 0u;
 }
 
 int cimba_b200_launch(const cimba_b200_device_job *job, void *stream)
@@ -460,433 +698,22 @@ int cimba_b200_launch(const cimba_b200_device_job *job, void *stream)
     if ((job->arr_mean == nullptr || job->srv_mean == nullptr) && job->model != CIMBA_B200_MODEL_AWACS)
         return fail(CIMBA_B200_EINVAL, "arr_mean/srv_mean device arrays are required");
     if (job->num_objects >= 0xffffffffull) return fail(CIMBA_B200_EINVAL, "num_objects must be < 2^32-1");
-    const int mapping = job->mapping == 0 ? CIMBA_B200_MAP_LANE : job->mapping;
+    const int mapping = mapping_of(job);
     if (mapping != CIMBA_B200_MAP_LANE && mapping != CIMBA_B200_MAP_WARP)
         return fail(CIMBA_B200_EINVAL, "mapping must be CIMBA_B200_MAP_LANE or CIMBA_B200_MAP_WARP");
-    const bool trace = job->trace_cap > 0u;
-    if (trace && (job->trace_key == nullptr || job->trace_time == nullptr))
+    if (job->trace_cap > 0u && (job->trace_key == nullptr || job->trace_time == nullptr))
         return fail(CIMBA_B200_EINVAL, "trace_cap > 0 needs trace_key and trace_time");
     if (cimba_b200_device_count() <= 0) return fail(CIMBA_B200_ENODEVICE, "no CUDA device");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (spill_cap_of(job) == 0xffffffffu)
+    if (cmb::spill_cap(*job) == 0u)
         return fail(CIMBA_B200_EINVAL, "queue_spill_cap must be 0 (default) or a power of two <= 2^26");
     if (job->num_params > CIMBA_B200_MAX_MODEL_PARAMS || (job->num_params > 0u && job->params == nullptr))
         return fail(CIMBA_B200_EINVAL, "params: at most CIMBA_B200_MAX_MODEL_PARAMS doubles behind a HOST pointer");
 
-    if (job->model >= CIMBA_B200_MODEL_USER_BASE) {
-        const UserModel *um = user_model(job->model);
-        if (um == nullptr) return fail(CIMBA_B200_EINVAL, "unknown model id (cimba_b200_model_load returns the ids of loaded models)");
-        if (job->workspace_bytes < um->workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        const int e = um->launch(job, stream);
-        g_launches++;
-        return e == 0 ? CIMBA_B200_OK : cuda_fail((cudaError_t)e, um->name.c_str());
-    }
-    if (goes_static(job)) {
-        if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "the static tier runs one trial per lane (CIMBA_B200_MAP_LANE)");
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        const int e = job->model == CIMBA_B200_MODEL_TUTORIAL1 ? cmb::launch_static_model<models::Tutorial1T, 2, 0, 3>(*job, st)
-                    : job->model == CIMBA_B200_MODEL_MM1 ? cmb::launch_static_model<models::MM1T, 2, 1>(*job, st)
-                    : job->model == CIMBA_B200_MODEL_GG1 ? cmb::launch_static_model<models::GG1T, 2, 1>(*job, st)
-                                                         : cmb::launch_static_model<models::MM1RecordedT, 2, 1>(*job, st);
-        g_launches += job->status != nullptr ? 2 : 1;
-        return e == 0 ? CIMBA_B200_OK : cuda_fail((cudaError_t)e, "static_trial_kernel launch");
-    }
-    if (coverage_goes_general(job)) {
-        if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "the general engine runs one trial per lane (CIMBA_B200_MAP_LANE)");
-        const bool no_capacity = job->model == CIMBA_B200_MODEL_TIMERS || job->model == CIMBA_B200_MODEL_RESOURCE_RECORDED;
-        if (!no_capacity && job->servers < 1) return fail(CIMBA_B200_EINVAL, "capacity (servers) must be >= 1");
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        return for_coverage_model<LaunchOf>(job->model, job, (unsigned char *)job->workspace, job->workspace_bytes, 0u, st);
-    }
-    if (job->model == CIMBA_B200_MODEL_RENEGE || job->model == CIMBA_B200_MODEL_POOL_RECORDED || job->model == CIMBA_B200_MODEL_TUTORIAL1 || job->model == CIMBA_B200_MODEL_PARK || job->model == CIMBA_B200_MODEL_TUTORIAL2 || mmc_goes_general(job) || fast_goes_general(job) || hold_goes_general(job) || harbor_goes_general(job)) {
-        if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "the general engine runs one trial per lane (CIMBA_B200_MAP_LANE)");
-        if (job->servers < 1) return fail(CIMBA_B200_EINVAL, "servers must be >= 1");
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        unsigned char *ws = (unsigned char *)job->workspace;
-        if (job->model == CIMBA_B200_MODEL_RENEGE)
-            return launch_general<models::Renege>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<Renege> launch");
-        if (job->model == CIMBA_B200_MODEL_TUTORIAL2)
-            return launch_general<models::Tutorial2>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<Tutorial2> launch");
-        if (job->model == CIMBA_B200_MODEL_PARK)
-            return launch_general<models::Park>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<Park> launch");
-        if (job->model == CIMBA_B200_MODEL_TUTORIAL1)
-            return launch_general<models::Tutorial1>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<Tutorial1> launch");
-        if (job->model == CIMBA_B200_MODEL_POOL_RECORDED)
-            return launch_general<models::Cheese>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<Cheese> launch");
-        if (job->model == CIMBA_B200_MODEL_MMC)
-            return launch_general<models::MMC>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<MMC> launch");
-        if (job->model == CIMBA_B200_MODEL_HOLD)
-            return launch_general<models::HoldGeneral>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<HoldGeneral> launch");
-        if (job->model == CIMBA_B200_MODEL_HARBOR) {
-            if (job->servers < 3) return fail(CIMBA_B200_EINVAL, "tugs (servers) must be >= 3 for CIMBA_B200_MODEL_HARBOR (a large ship needs 3)");
-            return launch_general<models::HarborGeneral>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<HarborGeneral> launch");
-        }
-        if (job->model == CIMBA_B200_MODEL_MM1)
-            return launch_general<models::MM1>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<MM1> launch");
-        if (job->model == CIMBA_B200_MODEL_MM1_RECORDED)
-            return launch_general<models::MM1Recorded>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<MM1Recorded> launch");
-        return launch_general<models::GG1>(job, ws, job->workspace_bytes, 0u, st, "trial_kernel<GG1> launch");
-    }
-
-    if (is_queue_model(job->model)) {
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        QueueArgs qa{};
-        qa.mapping = mapping;
-        qa.master_seed = job->master_seed;
-        qa.first_trial = job->first_trial;
-        qa.num_trials = job->num_trials;
-        qa.num_objects = job->num_objects;
-        qa.arr_mean = job->arr_mean;
-        qa.srv_mean = job->srv_mean;
-        qa.events = job->events;
-        qa.objects = job->objects;
-        qa.t_end = job->t_end;
-        qa.sum_wait = job->sum_wait;
-        qa.status = job->status;
-        qa.max_queue = job->max_queue;
-        qa.counters = job->counters;
-        qa.spill = (double *)job->workspace;
-        qa.spill_cap = spill_cap_of(job);
-        qa.trace_cap = job->trace_cap;
-        qa.trace_key = job->trace_key;
-        qa.trace_time = job->trace_time;
-        qa.diag = (unsigned long long *)job->diag;
-        const uint64_t threads = job->num_trials * (uint64_t)mapping;
-        const uint64_t blocks = (threads + QUEUE_BLOCK - 1) / QUEUE_BLOCK;
-        if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
-        dim3 grid((unsigned)blocks);
-        if (job->model == CIMBA_B200_MODEL_GG1) {
-            if (job->variant == 1) return launch_queue<1>(qa, trace, grid, st);
-            if (trace) gg1_kernel<true><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
-            else       gg1_kernel<false><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
-            g_launches++;
-            cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return cuda_fail(e, "gg1_kernel launch");
-            if (job->status == nullptr) return CIMBA_B200_OK;       // nobody could see a flag: nothing to repair by
-            return launch_general<models::GG1>(job, (unsigned char *)job->workspace + align256(job->num_trials * (uint64_t)qa.spill_cap * sizeof(double)),
-                                               repair_arena_bytes(job), REPAIR_BITS, st, "repair pass (G/G/1)");
-        }
-        if (job->model == CIMBA_B200_MODEL_MM1_RECORDED) {
-            if (job->counters == nullptr)
-                return fail(CIMBA_B200_EINVAL, "CIMBA_B200_MODEL_MM1_RECORDED writes its cmb_wtdsummary to counters[]");
-            if (trace) queue_kernel<0, true, true><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
-            else       queue_kernel<0, false, true><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
-            g_launches++;
-            cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return cuda_fail(e, "queue_kernel (recorded) launch");
-            if (job->status == nullptr) return CIMBA_B200_OK;
-            return launch_general<models::MM1Recorded>(job, (unsigned char *)job->workspace + align256(job->num_trials * (uint64_t)qa.spill_cap * sizeof(double)),
-                                                       repair_arena_bytes(job), REPAIR_BITS, st, "repair pass (M/M/1 with its queue history)");
-        }
-        if (job->variant == 1) return launch_queue<0>(qa, trace, grid, st);
-        if (job->variant == 2) {                        // variates from producer warps (mm1_pc.cuh): an experiment, same answers
-            if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "variant 2 of MODEL_MM1 runs one trial per lane");
-            const dim3 pc_grid((unsigned)((job->num_trials + MM1_PC_CONSUMERS - 1) / MM1_PC_CONSUMERS));
-            if (trace) mm1_pc_kernel<true><<<pc_grid, 2 * MM1_PC_CONSUMERS, 0, st>>>(qa);
-            else       mm1_pc_kernel<false><<<pc_grid, 2 * MM1_PC_CONSUMERS, 0, st>>>(qa);
-        }
-        else if (trace) {
-            mm1_kernel<true><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
-        }
-        else {
-            mm1_kernel<false><<<grid, QUEUE_BLOCK, 0, st>>>(qa);
-        }
-        g_launches++;
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return cuda_fail(e, "mm1_kernel launch");
-        if (job->status == nullptr) return CIMBA_B200_OK;           // nobody could see a flag: nothing to repair by
-        return launch_general<models::MM1>(job, (unsigned char *)job->workspace + align256(job->num_trials * (uint64_t)qa.spill_cap * sizeof(double)),
-                                           repair_arena_bytes(job), REPAIR_BITS, st, "repair pass (M/M/1)");
-    }
-    if (job->model == CIMBA_B200_MODEL_MMC) {
-        if (job->servers < 1) return fail(CIMBA_B200_EINVAL, "servers must be >= 1 for CIMBA_B200_MODEL_MMC");
-        if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "MODEL_MMC supports CIMBA_B200_MAP_LANE only");
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        PoolArgs pa{};
-        pa.servers = job->servers;
-        pa.master_seed = job->master_seed;
-        pa.first_trial = job->first_trial;
-        pa.num_trials = job->num_trials;
-        pa.num_objects = job->num_objects;
-        pa.arr_mean = job->arr_mean;
-        pa.srv_mean = job->srv_mean;
-        pa.events = job->events;
-        pa.objects = job->objects;
-        pa.t_end = job->t_end;
-        pa.sum_wait = job->sum_wait;
-        pa.status = job->status;
-        pa.max_queue = job->max_queue;
-        pa.spill = (double *)job->workspace;
-        pa.spill_cap = spill_cap_of(job);
-        pa.trace_cap = job->trace_cap;
-        pa.trace_key = job->trace_key;
-        pa.trace_time = job->trace_time;
-        pa.diag = (unsigned long long *)job->diag;
-        const uint64_t blocks = (job->num_trials + POOL_BLOCK - 1) / POOL_BLOCK;
-        if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
-        if (job->variant == 1) {                        // the readable formulation, pool_model.cuh
-            if (trace) pool_kernel<true><<<(unsigned)blocks, POOL_BLOCK, 0, st>>>(pa);
-            else       pool_kernel<false><<<(unsigned)blocks, POOL_BLOCK, 0, st>>>(pa);
-        }
-        else if (trace) {
-            pool_fast_kernel<true><<<(unsigned)blocks, POOL_BLOCK, 0, st>>>(pa);
-        }
-        else {
-            pool_fast_kernel<false><<<(unsigned)blocks, POOL_BLOCK, 0, st>>>(pa);
-        }
-        g_launches++;
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return cuda_fail(e, "pool_kernel launch");
-        if (job->status == nullptr) return CIMBA_B200_OK;
-        return launch_general<models::MMC>(job, (unsigned char *)job->workspace + align256(job->num_trials * (uint64_t)pa.spill_cap * sizeof(double)),
-                                           repair_arena_bytes(job), REPAIR_BITS, st, "repair pass (M/M/c)");
-    }
-    if (is_general_model(job->model)) {
-        const bool rsc = job->model == CIMBA_B200_MODEL_RESOURCE_RECORDED;
-        const bool tmr = job->model == CIMBA_B200_MODEL_TIMERS || rsc;      // no capacity argument
-        const bool prq = job->model == CIMBA_B200_MODEL_PRIOQ;
-        const bool pre = job->model == CIMBA_B200_MODEL_PREEMPT;
-        const bool buf = job->model == CIMBA_B200_MODEL_BUFFER || job->model == CIMBA_B200_MODEL_BUFFER_RECORDED;
-        const bool pq13 = job->model == CIMBA_B200_MODEL_PRIOQ_RECORDED;
-        if (!tmr && job->servers < 1) return fail(CIMBA_B200_EINVAL, "capacity (servers) must be >= 1");
-        if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "MODEL_GUARDED supports CIMBA_B200_MAP_LANE only");
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        GuardedArgs ga{};
-        ga.capacity = job->servers;
-        ga.master_seed = job->master_seed;
-        ga.first_trial = job->first_trial;
-        ga.num_trials = job->num_trials;
-        ga.duration = job->num_objects;
-        ga.put_mean = job->arr_mean;
-        ga.get_mean = job->srv_mean;
-        ga.events = job->events;
-        ga.objects = job->objects;
-        ga.t_end = job->t_end;
-        ga.sum_wait = job->sum_wait;
-        ga.status = job->status;
-        ga.max_queue = job->max_queue;
-        ga.counters = job->counters;
-        ga.state = (GeneralState *)job->workspace;
-        ga.record = (job->model == CIMBA_B200_MODEL_GUARDED_RECORDED || job->model == CIMBA_B200_MODEL_BUFFER_RECORDED ||
-                     job->model == CIMBA_B200_MODEL_PRIOQ_RECORDED) ? 1u : 0u;
-        ga.use_pq = job->model == CIMBA_B200_MODEL_PRIOQ_RECORDED ? 1u : 0u;
-        ga.trace_cap = job->trace_cap;
-        ga.trace_key = job->trace_key;
-        ga.trace_time = job->trace_time;
-        const uint64_t blocks = (job->num_trials + GUARDED_BLOCK - 1) / GUARDED_BLOCK;
-        if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
-        if (rsc) {
-            if (trace) resource_kernel<true><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-            else       resource_kernel<false><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-        }
-        else if (tmr) {
-            if (trace) timers_kernel<true><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-            else       timers_kernel<false><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-        }
-        else if (prq) {
-            if (trace) prioq_kernel<true><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-            else       prioq_kernel<false><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-        }
-        else if (buf) {
-            if (trace) buffer_kernel<true><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-            else       buffer_kernel<false><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-        }
-        else if (pre) {
-            if (trace) preempt_kernel<true><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-            else       preempt_kernel<false><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-        }
-        else if (trace) {
-            guarded_kernel<true><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-        }
-        else {
-            guarded_kernel<false><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ga);
-        }
-        g_launches++;
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return cuda_fail(e, "guarded_kernel launch");
-        if (job->status == nullptr) return CIMBA_B200_OK;
-        return for_coverage_model<LaunchOf>(job->model, job, (unsigned char *)job->workspace + align256(job->num_trials * (uint64_t)sizeof(GeneralState)),
-                                            repair_arena_bytes(job), REPAIR_BITS, st);
-    }
-    if (job->model == CIMBA_B200_MODEL_HARBOR) {
-        if (job->servers < 3 || job->servers > 255)
-            return fail(CIMBA_B200_EINVAL, "tugs (servers) must be in 3..255 for CIMBA_B200_MODEL_HARBOR (a large ship needs 3)");
-        if (mapping != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "MODEL_HARBOR supports CIMBA_B200_MAP_LANE only");
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        HarborArgs ha{};
-        ha.tugs = job->servers;
-        ha.master_seed = job->master_seed;
-        ha.first_trial = job->first_trial;
-        ha.num_trials = job->num_trials;
-        ha.duration = job->num_objects;
-        ha.arr_mean = job->arr_mean;
-        ha.unload_small = job->srv_mean;
-        ha.events = job->events;
-        ha.objects = job->objects;
-        ha.t_end = job->t_end;
-        ha.sum_wait = job->sum_wait;
-        ha.status = job->status;
-        ha.max_queue = job->max_queue;
-        ha.counters = job->counters;
-        ha.state = job->workspace;
-        ha.trace_cap = job->trace_cap;
-        ha.trace_key = job->trace_key;
-        ha.trace_time = job->trace_time;
-        // variant 0: up to 32 768 trials run warp-per-trial with the state in shared memory, and whatever trial
-        // outgrew those tables is re-run by the lane-per-trial kernel with the large HBM-resident tables; more
-        // trials go lane-per-trial directly.  (H100, 400 W, 600 h per trial: warp-per-trial 44 / 154 / 299 ms
-        // at 4096 / 16 384 / 32 768 trials, lane-per-trial 151 / 200 / 406 ms.)
-        // variant 1 = warp-per-trial only (overflow -> status), variant 2 = lane-per-trial only.
-        const bool on_chip_first = job->variant == 1 ||
-                                   (job->variant == 0 && job->num_trials <= 32768u && job->status != nullptr);
-        ha.repair = 0u;
-        if (on_chip_first) {
-            const size_t smem = (HARBOR_BLOCK_ON_CHIP / 32) * sizeof(HarborStateOnChip);
-            const void *fn = trace ? (const void *)harbor_on_chip_kernel<true> : (const void *)harbor_on_chip_kernel<false>;
-            CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            int dev = 0, sms = 132, per_sm = 0;
-            CUDA_TRY(cudaGetDevice(&dev));
-            CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-            cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, HARBOR_BLOCK_ON_CHIP, smem);
-            if (oe != cudaSuccess || per_sm < 1) per_sm = 4;
-            const uint64_t per_block = HARBOR_BLOCK_ON_CHIP / 32;
-            const uint64_t resident = (uint64_t)sms * (uint64_t)per_sm;
-            const uint64_t wanted = (job->num_trials + per_block - 1) / per_block;
-            const unsigned nb = (unsigned)(wanted < resident ? wanted : resident);
-            void *kargs[] = { (void *)&ha };
-            cudaError_t le = cudaLaunchKernel(fn, dim3(nb), dim3(HARBOR_BLOCK_ON_CHIP), kargs, smem, st);
-            g_launches++;
-            cudaError_t e2 = le != cudaSuccess ? le : cudaGetLastError();
-            if (e2 != cudaSuccess) return cuda_fail(e2, "harbor_on_chip_kernel launch");
-            if (job->variant == 1) return CIMBA_B200_OK;
-            ha.repair = 1u;
-        }
-        const uint64_t blocks = (job->num_trials + GUARDED_BLOCK - 1) / GUARDED_BLOCK;
-        if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
-        if (trace) harbor_kernel<true><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ha);
-        else       harbor_kernel<false><<<(unsigned)blocks, GUARDED_BLOCK, 0, st>>>(ha);
-        g_launches++;
-        cudaError_t e = cudaGetLastError();
-        return e == cudaSuccess ? CIMBA_B200_OK : cuda_fail(e, "harbor_kernel launch");
-    }
-    if (job->model == CIMBA_B200_MODEL_AWACS) {
-        if (job->num_objects == 0u) return fail(CIMBA_B200_EINVAL, "MODEL_AWACS: num_objects = trial duration in seconds, > 0");
-        if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-            return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-        int dev = 0;
-        CUDA_TRY(cudaGetDevice(&dev));
-        AwacsArgs aa{};
-        {
-            std::lock_guard<std::mutex> hold(g_terrain_mu);
-            if (dev < 0 || dev >= MAX_TERRAIN_DEVICES || !g_terrain_set[dev])
-                return fail(CIMBA_B200_EINVAL, "MODEL_AWACS: no terrain registered on this device; call cimba_b200_awacs_set_terrain()");
-            aa.ter = g_terrain[dev];
-        }
-        aa.orbit = awacs_orbit();
-        aa.master_seed = job->master_seed;
-        aa.first_trial = job->first_trial;
-        aa.num_trials = job->num_trials;
-        aa.t_end_s = (double)job->num_objects;
-        aa.state = (unsigned char *)job->workspace;
-        aa.events = job->events;
-        aa.objects = job->objects;
-        aa.t_end = job->t_end;
-        aa.sum_wait = job->sum_wait;
-        aa.status = job->status;
-        aa.max_queue = job->max_queue;
-        aa.counters = job->counters;
-        aa.trace_cap = job->trace_cap;
-        aa.trace_key = job->trace_key;
-        aa.trace_time = job->trace_time;
-        const uint64_t per_block = AWACS_BLOCK / 32;
-        const uint64_t blocks = (job->num_trials + per_block - 1) / per_block;
-        if (blocks > 0x7fffffffull) return fail(CIMBA_B200_EINVAL, "too many trials for one launch");
-        if (trace) awacs_kernel<true><<<(unsigned)blocks, AWACS_BLOCK, 0, st>>>(aa);
-        else       awacs_kernel<false><<<(unsigned)blocks, AWACS_BLOCK, 0, st>>>(aa);
-        g_launches++;
-        cudaError_t e = cudaGetLastError();
-        return e == cudaSuccess ? CIMBA_B200_OK : cuda_fail(e, "awacs_kernel launch");
-    }
-    if (job->model == CIMBA_B200_MODEL_HOLD) {
-        const bool on_chip = job->variant == 1;         // hold_model.cuh: the whole list in shared memory
-        if (job->servers < 1 || (on_chip && job->servers > HOLD_CAP - 8) ||
-            (uint32_t)job->servers + 2u > DEEP_MAX_ENTRIES)
-            return fail(CIMBA_B200_EINVAL, "workers (servers) must be in 1..33822 for CIMBA_B200_MODEL_HOLD (1..1080 with variant 1)");
-        HoldArgs ha{};
-        ha.workers = job->servers;
-        ha.master_seed = job->master_seed;
-        ha.first_trial = job->first_trial;
-        ha.num_trials = job->num_trials;
-        ha.duration = job->num_objects;
-        ha.mean = job->arr_mean;
-        ha.events = job->events;
-        ha.objects = job->objects;
-        ha.t_end = job->t_end;
-        ha.sum_wait = job->sum_wait;
-        ha.status = job->status;
-        ha.max_queue = job->max_queue;
-        ha.counters = job->counters;
-        ha.trace_cap = job->trace_cap;
-        ha.trace_key = job->trace_key;
-        ha.trace_time = job->trace_time;
-        if (!on_chip) {
-            // hold_deep.cuh: levels >= 2 of the 32-ary heap in HBM/L2, persistent warps
-            if (job->workspace_bytes < cimba_b200_workspace_bytes(job) || job->workspace == nullptr)
-                return fail(CIMBA_B200_EINVAL, "workspace too small; see cimba_b200_workspace_bytes()");
-            // variant 0 = the default below; 2 = one warp per trial (hold_deep.cuh); 3 / 4 = 16 / 8 lanes per trial
-            const int lanes = job->variant == 2 ? 32 : (job->variant == 4 ? 8 : (job->variant == 3 ? 16 : HOLD_DEFAULT_LANES));
-            const void *fn = lanes == 32 ? (trace ? (const void *)hold_deep_kernel<true> : (const void *)hold_deep_kernel<false>)
-                           : lanes == 16 ? (trace ? (const void *)hold_group_kernel<16, true> : (const void *)hold_group_kernel<16, false>)
-                                         : (trace ? (const void *)hold_group_kernel<8, true> : (const void *)hold_group_kernel<8, false>);
-            int dev = 0, sms = 132, per_sm = 0;
-            CUDA_TRY(cudaGetDevice(&dev));
-            CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-            cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, DEEP_BLOCK, 0);
-            if (oe != cudaSuccess || per_sm < 1) per_sm = 8;
-            const uint64_t trials_per_block = (uint64_t)(DEEP_BLOCK / 32) * (uint64_t)(32 / lanes);
-            const uint64_t resident = (uint64_t)sms * (uint64_t)per_sm;
-            const uint64_t wanted = (job->num_trials + trials_per_block - 1) / trials_per_block;
-            const unsigned blocks = (unsigned)(wanted < resident ? wanted : resident);
-            DeepArgs da{};
-            da.h = ha;
-            da.rows = (uint4 *)job->workspace;
-            da.row_entries = deep_row_entries(job->servers);
-            void *kargs[] = { (void *)&da };
-            cudaError_t le = cudaLaunchKernel(fn, dim3(blocks), dim3(DEEP_BLOCK), kargs, 0, st);
-            g_launches++;
-            cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
-            return e == cudaSuccess ? CIMBA_B200_OK : cuda_fail(e, "hold_deep_kernel launch");
-        }
-        // persistent one-warp CTAs: exactly as many as are resident at once (shared memory
-        // bounds it at ~12 per SM), so no CTA waits for another to retire
-        int dev = 0, sms = 132, per_sm = 0;
-        CUDA_TRY(cudaGetDevice(&dev));
-        CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        cudaError_t oe = trace
-            ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hold_kernel<true>, 32, HOLD_SMEM_BYTES)
-            : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hold_kernel<false>, 32, HOLD_SMEM_BYTES);
-        if (oe != cudaSuccess || per_sm < 1) per_sm = 8;
-        const uint64_t resident = (uint64_t)sms * (uint64_t)per_sm;
-        const unsigned blocks = (unsigned)(job->num_trials < resident ? job->num_trials : resident);
-        if (trace) {
-            hold_kernel<true><<<blocks, 32, HOLD_SMEM_BYTES, st>>>(ha);
-        }
-        else {
-            hold_kernel<false><<<blocks, 32, HOLD_SMEM_BYTES, st>>>(ha);
-        }
-        g_launches++;
-        cudaError_t e = cudaGetLastError();
-        return e == cudaSuccess ? CIMBA_B200_OK : cuda_fail(e, "hold_kernel launch");
-    }
-    return fail(CIMBA_B200_EINVAL, "unknown model");
+    const Route *r = route(job);
+    if (r == nullptr)
+        return fail(CIMBA_B200_EINVAL, job->model >= CIMBA_B200_MODEL_USER_BASE
+                                           ? "unknown model id (cimba_b200_model_load returns the ids of loaded models)" : "unknown model");
+    return r->launch(job, (cudaStream_t)stream);
 }
 
 namespace {

@@ -34,6 +34,60 @@ struct ArenaNeed<Model, decltype((void)Model::arena_bytes_per_trial(*(const cimb
 
 constexpr uint64_t ARENA_HEADER = 256u;         // the allocation cursor lives in front of the arena
 
+// What a fixed-capacity kernel flags (its queue, event list, wait lists or process table outgrew their tables) is re-run
+// on the general engine, whose containers grow, by a repair pass inside the same launch.
+constexpr uint32_t REPAIR_BITS = CIMBA_B200_TRIAL_QUEUE_OVERFLOW | CIMBA_B200_TRIAL_FEL_OVERFLOW |
+                                 CIMBA_B200_TRIAL_GUARD_OVERFLOW | CIMBA_B200_TRIAL_PROC_OVERFLOW;
+
+constexpr uint32_t SPILL_CAP_DEFAULT = 512u;    // HBM ring entries per queue and trial behind the on-chip window
+
+// job.queue_spill_cap: 0 = the default, else a power of two up to 2^26; 0 = invalid
+inline uint32_t spill_cap(const cimba_b200_device_job &job)
+{
+    const uint64_t c = job.queue_spill_cap;
+    if (c == 0u) return SPILL_CAP_DEFAULT;
+    return (c & (c - 1u)) == 0u && c <= (1ull << 26) ? (uint32_t)c : 0u;
+}
+
+inline uint64_t align256(uint64_t v) { return (v + 255u) & ~(uint64_t)255u; }
+
+// The workspace of a fixed-capacity kernel: its rings, then (256-byte aligned) the growth arena of its repair pass
+inline uint64_t rings_then_arena(uint64_t rings_bytes, uint64_t arena_bytes) { return align256(rings_bytes) + arena_bytes; }
+
+// The fields every kernel argument struct has, from the job; the caller fills the rest
+template <class Args>
+Args job_args(const cimba_b200_device_job &job)
+{
+    Args a{};
+    a.master_seed = job.master_seed;
+    a.first_trial = job.first_trial;
+    a.num_trials = job.num_trials;
+    a.events = job.events;
+    a.objects = job.objects;
+    a.t_end = job.t_end;
+    a.sum_wait = job.sum_wait;
+    a.status = job.status;
+    a.max_queue = job.max_queue;
+    a.trace_cap = job.trace_cap;
+    a.trace_key = job.trace_key;
+    a.trace_time = job.trace_time;
+    return a;
+}
+
+inline LaunchArgs launch_args(const cimba_b200_device_job &job)
+{
+    LaunchArgs a = job_args<LaunchArgs>(job);
+    a.num_objects = job.num_objects;
+    a.servers = job.servers;
+    a.arr_mean = job.arr_mean;
+    a.srv_mean = job.srv_mean;
+    a.counters = job.counters;
+    a.diag = (unsigned long long *)job.diag;
+    a.num_params = job.params != nullptr ? (job.num_params < 16u ? job.num_params : 16u) : 0u;
+    for (uint32_t k = 0; k < a.num_params; k++) a.params[k] = job.params[k];
+    return a;
+}
+
 template <class Model>
 uint64_t workspace_bytes_for(const cimba_b200_device_job &job)
 {
@@ -48,30 +102,10 @@ int launch_model(const cimba_b200_device_job &job, unsigned char *arena, uint64_
                  cudaStream_t stream)
 {
     if (arena == nullptr || arena_bytes <= ARENA_HEADER) return (int)cudaErrorInvalidValue;
-    LaunchArgs a{};
-    a.master_seed = job.master_seed;
-    a.first_trial = job.first_trial;
-    a.num_trials = job.num_trials;
-    a.num_objects = job.num_objects;
-    a.servers = job.servers;
+    LaunchArgs a = launch_args(job);
     a.only_flagged = only_flagged;
-    a.arr_mean = job.arr_mean;
-    a.srv_mean = job.srv_mean;
-    a.events = job.events;
-    a.objects = job.objects;
-    a.t_end = job.t_end;
-    a.sum_wait = job.sum_wait;
-    a.status = job.status;
-    a.max_queue = job.max_queue;
-    a.counters = job.counters;
     a.arena_base = arena;
     a.arena_bytes = arena_bytes - ARENA_HEADER;
-    a.trace_cap = job.trace_cap;
-    a.trace_key = job.trace_key;
-    a.trace_time = job.trace_time;
-    a.diag = (unsigned long long *)job.diag;
-    a.num_params = job.params != nullptr ? (job.num_params < 16u ? job.num_params : 16u) : 0u;
-    for (uint32_t k = 0; k < a.num_params; k++) a.params[k] = job.params[k];
 
     cudaError_t e = cudaMemsetAsync(arena, 0, ARENA_HEADER, stream);
     if (e != cudaSuccess) return (int)e;
@@ -99,60 +133,36 @@ int launch_model(const cimba_b200_device_job &job, unsigned char *arena, uint64_
     return (int)cudaGetLastError();
 }
 
-// ---- the static tier (cmb_static.cuh): ModelT<StaticSim<NPROC, NQUEUE>> first, ModelT<Sim> for what it flags
-constexpr uint32_t STATIC_REPAIR_BITS = CIMBA_B200_TRIAL_QUEUE_OVERFLOW | CIMBA_B200_TRIAL_FEL_OVERFLOW |
-                                        CIMBA_B200_TRIAL_GUARD_OVERFLOW | CIMBA_B200_TRIAL_PROC_OVERFLOW;
-
-inline uint32_t static_spill_cap(const cimba_b200_device_job &job)     // HBM ring entries per queue and trial (a power of two)
+// The repair pass behind a fixed-capacity kernel whose rings take `rings_bytes` at the front of the workspace
+template <class Model>
+int launch_repair(const cimba_b200_device_job &job, uint64_t rings_bytes, uint64_t arena_bytes, cudaStream_t stream)
 {
-    const uint64_t c = job.queue_spill_cap;
-    if (c == 0u) return 512u;
-    return (c & (c - 1u)) == 0u && c <= (1ull << 26) ? (uint32_t)c : 0u;
+    return launch_model<Model>(job, (unsigned char *)job.workspace + align256(rings_bytes), arena_bytes, REPAIR_BITS, stream);
 }
 
+// ---- the static tier (cmb_static.cuh): ModelT<StaticSim<NPROC, NQUEUE>> first, ModelT<Sim> for what it flags
 inline uint64_t static_rings_bytes(const cimba_b200_device_job &job, int nqueue)
 {
-    const uint64_t b = job.num_trials * (uint64_t)nqueue * static_spill_cap(job) * sizeof(double);
-    return (b + 255u) & ~(uint64_t)255u;
+    return align256(job.num_trials * (uint64_t)nqueue * spill_cap(job) * sizeof(double));
 }
 
 template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
 uint64_t workspace_bytes_static(const cimba_b200_device_job &job)
 {
-    // the rings of the static kernel, then the growth arena of its repair pass (a share of the trials, not all of them)
+    // the growth arena of the repair pass holds a share of the trials, not all of them
     const uint64_t arena = ARENA_HEADER + (job.num_trials / 8u + 256u) * ArenaNeed<ModelT<Sim>>::per_trial(job) + (64ull << 20);
-    return static_rings_bytes(job, NQUEUE) + arena;
+    return rings_then_arena(static_rings_bytes(job, NQUEUE), arena);
 }
 
 template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
 int launch_static_model(const cimba_b200_device_job &job, cudaStream_t stream)
 {
-    const uint32_t cap = static_spill_cap(job);
+    const uint32_t cap = spill_cap(job);
     const uint64_t rings = static_rings_bytes(job, NQUEUE);
     if (cap == 0u || job.workspace == nullptr || job.workspace_bytes < workspace_bytes_static<ModelT, NPROC, NQUEUE, NEVENT>(job))
         return (int)cudaErrorInvalidValue;
     StaticArgs sa{};
-    LaunchArgs &a = sa.base;
-    a.master_seed = job.master_seed;
-    a.first_trial = job.first_trial;
-    a.num_trials = job.num_trials;
-    a.num_objects = job.num_objects;
-    a.servers = job.servers;
-    a.arr_mean = job.arr_mean;
-    a.srv_mean = job.srv_mean;
-    a.events = job.events;
-    a.objects = job.objects;
-    a.t_end = job.t_end;
-    a.sum_wait = job.sum_wait;
-    a.status = job.status;
-    a.max_queue = job.max_queue;
-    a.counters = job.counters;
-    a.trace_cap = job.trace_cap;
-    a.trace_key = job.trace_key;
-    a.trace_time = job.trace_time;
-    a.diag = (unsigned long long *)job.diag;
-    a.num_params = job.params != nullptr ? (job.num_params < 16u ? job.num_params : 16u) : 0u;
-    for (uint32_t k = 0; k < a.num_params; k++) a.params[k] = job.params[k];
+    sa.base = launch_args(job);
     sa.spill = (double *)job.workspace;
     sa.spill_cap = cap;
     const uint64_t blocks = (job.num_trials + STATIC_BLOCK - 1) / STATIC_BLOCK;
@@ -165,7 +175,7 @@ int launch_static_model(const cimba_b200_device_job &job, cudaStream_t stream)
     if (e != cudaSuccess) return (int)e;
     e = cudaGetLastError();
     if (e != cudaSuccess || job.status == nullptr) return (int)e;      // nobody could see a flag: nothing to repair by
-    return launch_model<ModelT<Sim>>(job, (unsigned char *)job.workspace + rings, job.workspace_bytes - rings, STATIC_REPAIR_BITS, stream);
+    return launch_repair<ModelT<Sim>>(job, rings, job.workspace_bytes - rings, stream);
 }
 
 }  // namespace cmb
