@@ -371,6 +371,22 @@ int static_launch(const cimba_b200_device_job *job, cudaStream_t st)
 template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
 constexpr Route STATIC{static_workspace<ModelT, NPROC, NQUEUE, NEVENT>, static_launch<ModelT, NPROC, NQUEUE, NEVENT>};
 
+// ... for a model without queues whose other routes already size its jobs (models 14, 18, 21): the tier keeps no rings, and its
+// repair pass grows the general engine's containers in the workspace WORKSPACE asks for - so a job needs the same workspace
+// whichever variant serves it.  SERVERS: refuse servers < 1, as the model's general-engine route does.
+template <template <class> class ModelT, int NPROC, int NEVENT, uint64_t (*WORKSPACE)(const cimba_b200_device_job *), bool SERVERS>
+int static_launch_in(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (mapping_of(job) != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "the static tier runs one trial per lane (CIMBA_B200_MAP_LANE)");
+    if (SERVERS && job->servers < 1) return fail(CIMBA_B200_EINVAL, "servers must be >= 1");
+    if (const int e = check_workspace(job)) return e;
+    return counted(cmb::launch_static_trials<ModelT, NPROC, 0, NEVENT>(*job, st), "static_trial_kernel launch",
+                   job->status != nullptr ? 2 : 1);
+}
+
+template <template <class> class ModelT, int NPROC, int NEVENT, uint64_t (*WORKSPACE)(const cimba_b200_device_job *), bool SERVERS>
+constexpr Route STATIC_IN{WORKSPACE, static_launch_in<ModelT, NPROC, NEVENT, WORKSPACE, SERVERS>};
+
 // ---- the fused M/M/1, G/G/1 and M/M/c kernels: a queue window on chip, a ring per trial in HBM
 uint64_t queue_rings_bytes(const cimba_b200_device_job *job)
 {
@@ -650,9 +666,11 @@ const Route *route(const cimba_b200_device_job *job)
     case CIMBA_B200_MODEL_HARBOR:       return general ? &HARBOR_ENGINE : &HARBOR;
     case CIMBA_B200_MODEL_AWACS:        return &AWACS;
     case CIMBA_B200_MODEL_RENEGE:       return &ENGINE<models::Renege>;
-    case CIMBA_B200_MODEL_POOL_RECORDED: return &ENGINE<models::Cheese>;
+    case CIMBA_B200_MODEL_POOL_RECORDED:
+        return on_static ? &STATIC_IN<models::CheeseT, 6, 6, engine_workspace<models::Cheese>, true> : &ENGINE<models::Cheese>;
     case CIMBA_B200_MODEL_PARK:         return &ENGINE<models::Park>;
-    case CIMBA_B200_MODEL_TUTORIAL2:    return &ENGINE<models::Tutorial2>;
+    case CIMBA_B200_MODEL_TUTORIAL2:
+        return on_static ? &STATIC_IN<models::Tutorial2T, 8, 8, engine_workspace<models::Tutorial2>, true> : &ENGINE<models::Tutorial2>;
     case CIMBA_B200_MODEL_GUARDED:            return coverage_route<models::Guarded<false, false>>(job, 16);
     case CIMBA_B200_MODEL_GUARDED_RECORDED:   return coverage_route<models::Guarded<false, true>>(job, 16);
     case CIMBA_B200_MODEL_PRIOQ_RECORDED:     return coverage_route<models::Guarded<true, true>>(job, 15);
@@ -661,7 +679,8 @@ const Route *route(const cimba_b200_device_job *job)
     case CIMBA_B200_MODEL_BUFFER:             return coverage_route<models::Workshop<false>>(job, INT32_MAX);
     case CIMBA_B200_MODEL_BUFFER_RECORDED:    return coverage_route<models::Workshop<true>>(job, INT32_MAX);
     case CIMBA_B200_MODEL_TIMERS:             return coverage_route<models::FrontDesk>(job, INT32_MAX);
-    case CIMBA_B200_MODEL_RESOURCE_RECORDED:  return coverage_route<models::Tool>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_RESOURCE_RECORDED:
+        return on_static ? &STATIC_IN<models::ToolT, 4, 2, coverage_workspace, false> : coverage_route<models::Tool>(job, INT32_MAX);
     }
     return job->model >= CIMBA_B200_MODEL_USER_BASE && user_model(job->model) != nullptr ? &USER : nullptr;
 }

@@ -154,13 +154,14 @@ uint64_t workspace_bytes_static(const cimba_b200_device_job &job)
     return rings_then_arena(static_rings_bytes(job, NQUEUE), arena);
 }
 
+// The static kernel over the job's trials, then the repair pass in the workspace behind its rings: launch_static_model below,
+// or a route of the library that sizes the workspace itself (capi.cu)
 template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
-int launch_static_model(const cimba_b200_device_job &job, cudaStream_t stream)
+int launch_static_trials(const cimba_b200_device_job &job, cudaStream_t stream)
 {
     const uint32_t cap = spill_cap(job);
     const uint64_t rings = static_rings_bytes(job, NQUEUE);
-    if (cap == 0u || job.workspace == nullptr || job.workspace_bytes < workspace_bytes_static<ModelT, NPROC, NQUEUE, NEVENT>(job))
-        return (int)cudaErrorInvalidValue;
+    if (cap == 0u || job.workspace == nullptr || job.workspace_bytes <= rings + ARENA_HEADER) return (int)cudaErrorInvalidValue;
     StaticArgs sa{};
     sa.base = launch_args(job);
     sa.spill = (double *)job.workspace;
@@ -176,6 +177,14 @@ int launch_static_model(const cimba_b200_device_job &job, cudaStream_t stream)
     e = cudaGetLastError();
     if (e != cudaSuccess || job.status == nullptr) return (int)e;      // nobody could see a flag: nothing to repair by
     return launch_repair<ModelT<Sim>>(job, rings, job.workspace_bytes - rings, stream);
+}
+
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
+int launch_static_model(const cimba_b200_device_job &job, cudaStream_t stream)
+{
+    if (spill_cap(job) == 0u || job.workspace == nullptr || job.workspace_bytes < workspace_bytes_static<ModelT, NPROC, NQUEUE, NEVENT>(job))
+        return (int)cudaErrorInvalidValue;
+    return launch_static_trials<ModelT, NPROC, NQUEUE, NEVENT>(job, stream);
 }
 
 }  // namespace cmb

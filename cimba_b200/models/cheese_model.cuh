@@ -6,24 +6,32 @@
 // on the holders' tie-break by process address (SURVEY.md quirk 4): the test creates its processes one after the other, so
 // address order is creation order, which is what the index-based key (pid + 1) gives.
 // Oracle: the same test against the reference's API, oracle/ref_build/ref_driver.c model 18.
+// A template over the engine, as tutorial1_model.cuh: cmb::Sim, or the static tier's second form (static_interrupts: priorities,
+// interrupts, pre-emption; the pool named in static_holdables, so that the end event's stops drop the holdings there).
 #pragma once
 #include "../csrc/cmb_kernel.cuh"
+#include "../csrc/cmb_static.cuh"
 
 namespace cimba_b200 {
 namespace models {
 
-struct Cheese {
-    cmb::resourcepool cheese;
+template <class S>
+struct CheeseT {
+    typename S::recorded_resourcepool_type cheese;
     uint64_t successes;
     double   sum_time;
     enum : uint32_t { MOUSE, RAT, CAT };
     enum : uint32_t { END_EVENT = cmb::ACT_CMB_USER };
     static constexpr uint32_t MICE = 3u, RATS = 2u, RODENTS = 5u;
+    static constexpr bool static_interrupts = true;
+    static CMB_FN constexpr uint32_t static_kind(uint32_t i) { return i < MICE ? MOUSE : (i < RODENTS ? RAT : CAT); }
+    template <class F>
+    CMB_FN void static_holdables(F &&visit) { visit(cheese); }
 
     // one rodent: u[0] = amount held (the body's local), u[1] = the amount of the call in progress
-    CMB_FN void rodent(cmb::Sim &sim, uint32_t me, int64_t sig, bool rat)
+    CMB_FN void rodent(S &sim, uint32_t me, int64_t sig, bool rat)
     {
-        Cheese &m = *this;
+        CheeseT &m = *this;
         CMB_PROCESS_BEGIN
         sim.proc[me].u[0] = 0u;
         for (;;) {
@@ -59,9 +67,9 @@ struct Cheese {
         CMB_PROCESS_END
     }
 
-    CMB_FN void cat(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void cat(S &sim, uint32_t me, int64_t sig)
     {
-        Cheese &m = *this;
+        CheeseT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(1.0);
@@ -74,7 +82,7 @@ struct Cheese {
         CMB_PROCESS_END
     }
 
-    CMB_FN void run_trial(cmb::Sim &sim, const cmb::TrialIn &in)                // test_pool, :307-379
+    CMB_FN void run_trial(S &sim, const cmb::TrialIn &in)                // test_pool, :307-379
     {
         successes = 0u;
         sum_time = 0.0;
@@ -87,22 +95,22 @@ struct Cheese {
         (void)cmb_event_schedule(END_EVENT, cmb::NIL, 0, (double)in.num_objects, 0);
     }
 
-    CMB_FN void process(cmb::Sim &sim, uint32_t me, uint32_t kind, int64_t sig)
+    CMB_FN void process(S &sim, uint32_t me, uint32_t kind, int64_t sig)
     {
         if (kind == CAT) cat(sim, me, sig);
         else rodent(sim, me, sig, kind == RAT);
     }
 
-    CMB_FN void event(cmb::Sim &sim, uint32_t action, uint32_t, int64_t)       // end_sim_evt, :50-72
+    CMB_FN void event(S &sim, uint32_t action, uint32_t, int64_t)       // end_sim_evt, :50-72
     {
-        Cheese &m = *this;
+        CheeseT &m = *this;
         if (action == END_EVENT) {
             for (uint32_t i = 0u; i <= RODENTS; i++) cmb_process_stop(i, 0);
         }
     }
-    CMB_FN bool demand(cmb::Sim &, uint32_t, uint32_t, int32_t) { return false; }
+    CMB_FN bool demand(S &, uint32_t, uint32_t, int32_t) { return false; }
 
-    CMB_FN void finish(cmb::Sim &sim, cmb::TrialOut &out)
+    CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         cmb_resourcepool_stop_recording(cheese);
         const WtdAcc &h = cheese.history.acc;           // what cmb_timeseries_summarize makes of the stored history
@@ -119,6 +127,8 @@ struct Cheese {
         out.max_queue = (uint32_t)h.count;
     }
 };
+
+using Cheese = CheeseT<cmb::Sim>;       // on the static tier: CheeseT<cmb::StaticSimOf<CheeseT, 6, 0, 6>> (six processes, six spare event slots)
 
 }  // namespace models
 }  // namespace cimba_b200

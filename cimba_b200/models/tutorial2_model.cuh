@@ -8,23 +8,30 @@
 // index-based key gives here (SURVEY.md quirk 4) - and cmb_random_flip's cached bits outlive a trial.
 //   counters[0] = the random stream's next raw output after the run (a fingerprint of every draw), [1] = units in use at the end,
 //   [2] = successful acquires + pre-empts; objects = the same.
+// A template over the engine, as tutorial1_model.cuh: cmb::Sim, or the static tier's second form (static_interrupts).
 #pragma once
 #include "../csrc/cmb_kernel.cuh"
+#include "../csrc/cmb_static.cuh"
 
 namespace cimba_b200 {
 namespace models {
 
-struct Tutorial2 {
-    cmb::resourcepool cheese;
+template <class S>
+struct Tutorial2T {
+    typename S::resourcepool_type cheese;
     uint64_t successes;
     enum : uint32_t { MOUSE, RAT, CAT };
     enum : uint32_t { END_SIM = cmb::ACT_CMB_USER };
     static constexpr uint32_t MICE = 5u, RATS = 2u, CATS = 1u, RODENTS = 7u;
+    static constexpr bool static_interrupts = true;
+    static CMB_FN constexpr uint32_t static_kind(uint32_t i) { return i < MICE ? MOUSE : (i < RODENTS ? RAT : CAT); }
+    template <class F>
+    CMB_FN void static_holdables(F &&visit) { visit(cheese); }
 
     // mousefunc :59-127 / ratfunc :129-197; u[0] = amount_held, u[1] = the amount of the call in progress
-    CMB_FN void rodent(cmb::Sim &sim, uint32_t me, int64_t sig, bool rat)
+    CMB_FN void rodent(S &sim, uint32_t me, int64_t sig, bool rat)
     {
-        Tutorial2 &m = *this;
+        Tutorial2T &m = *this;
         CMB_PROCESS_BEGIN
         sim.proc[me].u[0] = 0u;
         for (;;) {
@@ -58,9 +65,9 @@ struct Tutorial2 {
         CMB_PROCESS_END
     }
 
-    CMB_FN void cat(cmb::Sim &sim, uint32_t me, int64_t sig)                    // catfunc, :199-224
+    CMB_FN void cat(S &sim, uint32_t me, int64_t sig)                    // catfunc, :199-224
     {
-        Tutorial2 &m = *this;
+        Tutorial2T &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(5.0);
@@ -72,14 +79,14 @@ struct Tutorial2 {
         CMB_PROCESS_END
     }
 
-    CMB_FN void pounce(cmb::Sim &sim)
+    CMB_FN void pounce(S &sim)
     {
         const uint32_t target = (uint32_t)cmb_random_dice(0, (long long)RODENTS - 1);
         const int64_t with = cmb_random_flip() ? CMB_PROCESS_INTERRUPTED : (int64_t)cmb_random_dice(10, 100);
         cmb_process_interrupt(target, with, 0);
     }
 
-    CMB_FN void run_trial(cmb::Sim &sim, const cmb::TrialIn &)                  // :226-271
+    CMB_FN void run_trial(S &sim, const cmb::TrialIn &)                  // :226-271
     {
         successes = 0u;
         cmb_resourcepool_initialize(cheese, 20u);
@@ -90,22 +97,22 @@ struct Tutorial2 {
         (void)cmb_event_schedule(END_SIM, cmb::NIL, 0, 100000.0, 0);
     }
 
-    CMB_FN void process(cmb::Sim &sim, uint32_t me, uint32_t kind, int64_t sig)
+    CMB_FN void process(S &sim, uint32_t me, uint32_t kind, int64_t sig)
     {
         if (kind == CAT) cat(sim, me, sig);
         else rodent(sim, me, sig, kind == RAT);
     }
 
-    CMB_FN void event(cmb::Sim &sim, uint32_t action, uint32_t, int64_t)       // end_sim_evt, :40-57
+    CMB_FN void event(S &sim, uint32_t action, uint32_t, int64_t)       // end_sim_evt, :40-57
     {
-        Tutorial2 &m = *this;
+        Tutorial2T &m = *this;
         if (action == END_SIM) {
             for (uint32_t i = 0u; i < RODENTS + CATS; i++) cmb_process_stop(i, 0);
         }
     }
-    CMB_FN bool demand(cmb::Sim &, uint32_t, uint32_t, int32_t) { return false; }
+    CMB_FN bool demand(S &, uint32_t, uint32_t, int32_t) { return false; }
 
-    CMB_FN void finish(cmb::Sim &sim, cmb::TrialOut &out)
+    CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         out.counters[0] = sim.rng.next();
         out.counters[1] = cmb_resourcepool_in_use(cheese);
@@ -114,6 +121,8 @@ struct Tutorial2 {
         out.sum_wait = 0.0;
     }
 };
+
+using Tutorial2 = Tutorial2T<cmb::Sim>; // on the static tier: Tutorial2T<cmb::StaticSimOf<Tutorial2T, 8, 0, 8>> (eight processes, eight spare event slots)
 
 }  // namespace models
 }  // namespace cimba_b200

@@ -6,10 +6,12 @@
 // 1..8 (model 5); PLAIN = true: test/test_buffer.c as it stands - three fillers, three drainers, amounts 1..15, the level
 // history on (model 12, golden file test/reference/buffer.txt).
 // Tool: test/test_resource.c as it stands - three targets with random priorities and a pre-empter (priority 0) on one
-// cmb_resource with its history on (model 14, golden file test/reference/resource.txt).
+// cmb_resource with its history on (model 14, golden file test/reference/resource.txt).  A template over the engine, as
+// tutorial1_model.cuh: cmb::Sim, or the static tier's second form (static_interrupts: priorities, pre-emption).
 // Oracle: oracle/ref_build/ref_driver.c run_buffer_trial / run_resource_trial (the counters are described there).
 #pragma once
 #include "../csrc/cmb_kernel.cuh"
+#include "../csrc/cmb_static.cuh"
 
 namespace cimba_b200 {
 namespace models {
@@ -165,16 +167,21 @@ struct Workshop {
     }
 };
 
-struct Tool {
-    cmb::resource res;
+template <class S>
+struct ToolT {
+    typename S::recorded_resource_type res;
     uint64_t counter[8];
     double   sum_wait;
     enum : uint32_t { TARGET, PREEMPTER };
     enum : uint32_t { END_EVENT = cmb::ACT_CMB_USER };
+    static constexpr bool static_interrupts = true;
+    static CMB_FN constexpr uint32_t static_kind(uint32_t i) { return i < 3u ? TARGET : PREEMPTER; }
+    template <class F>
+    CMB_FN void static_holdables(F &&visit) { visit(res); }
 
-    CMB_FN void target(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void target(S &sim, uint32_t me, int64_t sig)
     {
-        Tool &m = *this;
+        ToolT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_RESOURCE_ACQUIRE(res);
@@ -199,9 +206,9 @@ struct Tool {
         CMB_PROCESS_END
     }
 
-    CMB_FN void preempter(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void preempter(S &sim, uint32_t me, int64_t sig)
     {
-        Tool &m = *this;
+        ToolT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_RESOURCE_PREEMPT(res);
@@ -213,7 +220,7 @@ struct Tool {
         CMB_PROCESS_END
     }
 
-    CMB_FN void run_trial(cmb::Sim &sim, const cmb::TrialIn &in)
+    CMB_FN void run_trial(S &sim, const cmb::TrialIn &in)
     {
         for (uint32_t i = 0u; i < 8u; i++) counter[i] = 0u;
         sum_wait = 0.0;
@@ -227,22 +234,22 @@ struct Tool {
         (void)cmb_event_schedule(END_EVENT, cmb::NIL, 0, (double)in.num_objects, 0);
     }
 
-    CMB_FN void process(cmb::Sim &sim, uint32_t me, uint32_t kind, int64_t sig)
+    CMB_FN void process(S &sim, uint32_t me, uint32_t kind, int64_t sig)
     {
         if (kind == TARGET) target(sim, me, sig);
         else preempter(sim, me, sig);
     }
 
-    CMB_FN void event(cmb::Sim &sim, uint32_t action, uint32_t, int64_t)
+    CMB_FN void event(S &sim, uint32_t action, uint32_t, int64_t)
     {
-        Tool &m = *this;
+        ToolT &m = *this;
         if (action == END_EVENT) {
             for (uint32_t i = 0u; i < 4u; i++) cmb_process_stop(i, 0);
         }
     }
-    CMB_FN bool demand(cmb::Sim &, uint32_t, uint32_t, int32_t) { return false; }
+    CMB_FN bool demand(S &, uint32_t, uint32_t, int32_t) { return false; }
 
-    CMB_FN void finish(cmb::Sim &sim, cmb::TrialOut &out)
+    CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         cmb_resource_stop_recording(res);
         counter[3] = (uint64_t)__double_as_longlong(res.history.acc.m1);
@@ -252,6 +259,8 @@ struct Tool {
         out.sum_wait = sum_wait;
     }
 };
+
+using Tool = ToolT<cmb::Sim>;     // on the static tier: ToolT<cmb::StaticSimOf<ToolT, 4, 0, 2>> (four processes, two spare event slots)
 
 }  // namespace models
 }  // namespace cimba_b200

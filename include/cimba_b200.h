@@ -155,8 +155,10 @@ const char *cimba_b200_model_name(int model_id);
  * run by the general engine (growable event list, wait lists and queues; any number of servers).  The fast kernels' repair pass
  * and MODEL_MMC with more than 14 servers use it too. */
 #define CIMBA_B200_VARIANT_GENERAL 16
-/* CIMBA_B200_MODEL_MM1 / _GG1 from their authoring-surface source on the static tier (cimba_b200/csrc/cmb_static.cuh):
- * process records and event slots in registers, the queue in shared memory; what it flags is re-run on the general engine */
+/* CIMBA_B200_MODEL_MM1 / _GG1 / _MM1_RECORDED from their authoring-surface source on the static tier (cimba_b200/csrc/cmb_static.cuh):
+ * process records and event slots in registers, the queue in shared memory; what it flags is re-run on the general engine.
+ * Also CIMBA_B200_MODEL_RESOURCE_RECORDED, _POOL_RECORDED and _TUTORIAL2 on the tier's form with priorities, interrupts and
+ * pre-emption (same workspace as their default route; the default routes are unchanged) */
 #define CIMBA_B200_VARIANT_STATIC 17
 
 /* Error codes */
