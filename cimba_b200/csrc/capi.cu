@@ -522,6 +522,28 @@ const Route *coverage_route(const cimba_b200_device_job *job, int max_servers)
     return job->variant == CIMBA_B200_VARIANT_GENERAL || job->servers > max_servers ? &engine : &fast;
 }
 
+// The static tier for the reference's queue tests (models 3, 6, 11 and 13): a job asks for the workspace of its default route -
+// the fixed-capacity kernel's up to MAX servers, the general engine's above (coverage_route) - and the repair pass grows in all
+// of it.  The object queue keeps its on-chip window and no HBM ring: one that outgrows the window flags the trial.
+template <class Model, int MAX>
+uint64_t coverage_or_engine_workspace(const cimba_b200_device_job *job)
+{
+    return job->servers > MAX ? engine_workspace<Model>(job) : coverage_workspace(job);
+}
+
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT>
+int static_coverage_launch(const cimba_b200_device_job *job, cudaStream_t st)
+{
+    if (job->servers < 1) return fail(CIMBA_B200_EINVAL, "capacity (servers) must be >= 1");
+    if (mapping_of(job) != CIMBA_B200_MAP_LANE) return fail(CIMBA_B200_EINVAL, "the static tier runs one trial per lane (CIMBA_B200_MAP_LANE)");
+    if (const int e = check_workspace(job)) return e;
+    return counted(cmb::launch_static_trials<ModelT, NPROC, NQUEUE, NEVENT, false>(*job, st), "static_trial_kernel launch",
+                   job->status != nullptr ? 2 : 1);
+}
+
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT, int MAX>
+constexpr Route STATIC_COVERAGE{coverage_or_engine_workspace<ModelT<cmb::Sim>, MAX>, static_coverage_launch<ModelT, NPROC, NQUEUE, NEVENT>};
+
 // ---- the harbor: up to 32 768 trials warp-per-trial with the state in shared memory, the rest lane-per-trial in HBM
 uint64_t harbor_workspace(const cimba_b200_device_job *job) { return job->num_trials * (uint64_t)sizeof(HarborState); }
 
@@ -671,10 +693,14 @@ const Route *route(const cimba_b200_device_job *job)
     case CIMBA_B200_MODEL_PARK:         return &ENGINE<models::Park>;
     case CIMBA_B200_MODEL_TUTORIAL2:
         return on_static ? &STATIC_IN<models::Tutorial2T, 8, 8, engine_workspace<models::Tutorial2>, true> : &ENGINE<models::Tutorial2>;
-    case CIMBA_B200_MODEL_GUARDED:            return coverage_route<models::Guarded<false, false>>(job, 16);
-    case CIMBA_B200_MODEL_GUARDED_RECORDED:   return coverage_route<models::Guarded<false, true>>(job, 16);
-    case CIMBA_B200_MODEL_PRIOQ_RECORDED:     return coverage_route<models::Guarded<true, true>>(job, 15);
-    case CIMBA_B200_MODEL_PRIOQ:              return coverage_route<models::QueueAndTide>(job, 15);
+    case CIMBA_B200_MODEL_GUARDED:
+        return on_static ? &STATIC_COVERAGE<models::GuardedQueueT, 7, 1, 2, 16> : coverage_route<models::Guarded<false, false>>(job, 16);
+    case CIMBA_B200_MODEL_GUARDED_RECORDED:
+        return on_static ? &STATIC_COVERAGE<models::GuardedRecordedQueueT, 7, 1, 2, 16> : coverage_route<models::Guarded<false, true>>(job, 16);
+    case CIMBA_B200_MODEL_PRIOQ_RECORDED:
+        return on_static ? &STATIC_COVERAGE<models::GuardedPriorityQueueT, 7, 0, 2, 15> : coverage_route<models::Guarded<true, true>>(job, 15);
+    case CIMBA_B200_MODEL_PRIOQ:
+        return on_static ? &STATIC_COVERAGE<models::QueueAndTideT, 8, 0, 2, 15> : coverage_route<models::QueueAndTide>(job, 15);
     case CIMBA_B200_MODEL_PREEMPT:            return coverage_route<models::PoolFight>(job, INT32_MAX);   // no table sized by `servers`
     case CIMBA_B200_MODEL_BUFFER:             return coverage_route<models::Workshop<false>>(job, INT32_MAX);
     case CIMBA_B200_MODEL_BUFFER_RECORDED:    return coverage_route<models::Workshop<true>>(job, INT32_MAX);

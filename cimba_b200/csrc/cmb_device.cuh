@@ -515,6 +515,9 @@ struct Sim {
     using recorded_resourcepool_type = resourcepool;
     using resource_type = resource;
     using recorded_resource_type = resource;
+    using priorityqueue_type = priorityqueue;
+    using recorded_priorityqueue_type = priorityqueue;
+    using condition_type = condition;
     Sfc64          rng;
     const ZigHot  *hot;
     double         now;
@@ -1435,6 +1438,11 @@ CMB_FN_NOINLINE uint64_t priorityqueue_position(Sim &sim, priorityqueue &q, uint
     return ahead + 1u;
 }
 
+CMB_FN uint64_t priorityqueue_length(const priorityqueue &q) { return (uint64_t)q.queue.count; }
+
+// cmb_priorityqueue_cancel: the object leaves, no signal
+CMB_FN bool priorityqueue_cancel(Sim &sim, priorityqueue &q, uint64_t handle) { return q.queue.remove(sim.arena, handle); }
+
 // ------------------------------------------------------------------------------------------------ condition
 CMB_FN void condition_initialize(Sim &sim, condition &c) { sim.guard_init(c.guard, &c); }
 
@@ -1460,6 +1468,8 @@ CMB_FN_NOINLINE uint32_t condition_signal(Sim &sim, Model &m, condition &c)
 }
 
 // ------------------------------------------------------------------------------------------------ process end
+CMB_FN int64_t process_priority(const Sim &sim, uint32_t pid) { return (int64_t)sim.proc[pid].prio; }
+
 // cmi_process_drop_resources, src/cmb_process.c:507-527: every held resource through its drop
 template <class Model>
 CMB_FN_NOINLINE void drop_resources(Sim &sim, Model &m, uint32_t pid)
@@ -1759,7 +1769,7 @@ CMB_FN double draw_std_normal(Sim &sim) { return gp_std_normal(sim.rng, *sim.hot
 #define cmb_process_timer_set(dur, s)       (sim.timer_set(me, (dur), (s)))
 #define cmb_process_timer_cancel(handle)    (sim.timer_cancel(me, (handle)))
 #define cmb_process_timers_clear(pid)       (sim.timers_clear(pid))
-#define cmb_process_priority(pid)           ((int64_t)sim.proc[pid].prio)
+#define cmb_process_priority(pid)           (cimba_b200::cmb::process_priority(sim, (pid)))
 #define cmb_process_priority_set(pid, pri)  (cimba_b200::cmb::process_priority_set(sim, (pid), (pri)))
 #define cmb_random_flip()                   (cimba_b200::rnd_flip(sim.rng, sim.flips))
 #define cmb_resourcepool_held_by_process(rp, pid) (cimba_b200::cmb::resourcepool_held_by_process(sim, (rp), (pid)))
@@ -1785,9 +1795,9 @@ CMB_FN double draw_std_normal(Sim &sim) { return gp_std_normal(sim.rng, *sim.hot
 #define cmb_priorityqueue_initialize(q, cap) (cimba_b200::cmb::priorityqueue_initialize(sim, (q), (cap)))
 #define cmb_priorityqueue_recording_start(q) (cimba_b200::cmb::priorityqueue_recording_start(sim, (q)))
 #define cmb_priorityqueue_recording_stop(q)  (cimba_b200::cmb::priorityqueue_recording_stop(sim, (q)))
-#define cmb_priorityqueue_length(q)         ((uint64_t)(q).queue.count)
+#define cmb_priorityqueue_length(q)         (cimba_b200::cmb::priorityqueue_length(q))
 #define cmb_priorityqueue_position(q, h)    (cimba_b200::cmb::priorityqueue_position(sim, (q), (h)))
-#define cmb_priorityqueue_cancel(q, h)      ((q).queue.remove(sim.arena, (h)))
+#define cmb_priorityqueue_cancel(q, h)      (cimba_b200::cmb::priorityqueue_cancel(sim, (q), (h)))
 #define cmb_priorityqueue_reprioritize(q, h, pri) (cimba_b200::cmb::priorityqueue_reprioritize(sim, (q), (h), (pri)))
 #define cmb_objectqueue_recording_start(q)  (cimba_b200::cmb::objectqueue_recording_start(sim, (q)))
 #define cmb_objectqueue_recording_stop(q)   (cimba_b200::cmb::objectqueue_recording_stop(sim, (q)))

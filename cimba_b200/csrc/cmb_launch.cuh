@@ -155,17 +155,18 @@ uint64_t workspace_bytes_static(const cimba_b200_device_job &job)
 }
 
 // The static kernel over the job's trials, then the repair pass in the workspace behind its rings: launch_static_model below,
-// or a route of the library that sizes the workspace itself (capi.cu)
-template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0>
+// or a route of the library that sizes the workspace itself (capi.cu).  RINGS = false: the queues keep only their on-chip
+// window (a bounded queue that outgrows it flags the trial) and the whole workspace is the repair pass's.
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT = 0, bool RINGS = true>
 int launch_static_trials(const cimba_b200_device_job &job, cudaStream_t stream)
 {
     const uint32_t cap = spill_cap(job);
-    const uint64_t rings = static_rings_bytes(job, NQUEUE);
+    const uint64_t rings = RINGS ? static_rings_bytes(job, NQUEUE) : 0u;
     if (cap == 0u || job.workspace == nullptr || job.workspace_bytes <= rings + ARENA_HEADER) return (int)cudaErrorInvalidValue;
     StaticArgs sa{};
     sa.base = launch_args(job);
-    sa.spill = (double *)job.workspace;
-    sa.spill_cap = cap;
+    sa.spill = RINGS ? (double *)job.workspace : nullptr;
+    sa.spill_cap = RINGS ? cap : 0u;
     const uint64_t blocks = (job.num_trials + STATIC_BLOCK - 1) / STATIC_BLOCK;
     if (blocks == 0u || blocks > 0x7fffffffull) return (int)cudaErrorInvalidValue;
     const bool trace = job.trace_cap > 0u;

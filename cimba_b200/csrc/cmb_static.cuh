@@ -20,9 +20,13 @@
 // while it holds from one of them.  Its guards are then literal binary heaps in the reference's layout (the wait-list order is
 // not a strict weak order, SURVEY.md quirk 1, so the physical heap decides who is woken), its interrupts and pre-emptions take
 // the model's NEVENT spare event slots, and cmb_random_flip has its per-trial cache.
+// In either form a cmb_priorityqueue (S::priorityqueue_type, S::recorded_priorityqueue_type) is a table of STATIC_PQ_CAP objects
+// scanned under its strict order, and a cmb_condition (S::condition_type) a literal heap of waiters with their predicates, whose
+// wake-ups take the waiters' own event slots; a model that reports cmb::Sim's fel_high says `static constexpr bool
+// static_fel_high = true;` (StaticSimHigh).
 // What the tier does NOT have - process creation beyond NPROC, timers, and, without static_interrupts, priorities other than
 // 0, interrupts and pre-emption; a process that ends while it holds from two or more containers, or from any without the hook;
-// a queue that outgrows window + ring, a spare slot or a guard heap too few - is not an error: the trial is flagged and the
+// a queue that outgrows window + ring or its table, a spare slot or a guard heap too few - is not an error: the trial is flagged and the
 // launch re-runs it on the general engine from the SAME model template (launch_static_model below), so the answer is the
 // reference's either way.
 //
@@ -30,7 +34,9 @@
 // `typename S::queue_type`, exported with CMB_EXPORT_STATIC_MODEL(M, NPROC, NQUEUE, "name") (or ..._EVENTS(M, NPROC, NQUEUE,
 // NEVENT, "name")).  In this library: mm1_model.cuh, gg1_model.cuh, mm1_recorded_model.cuh, tutorial1_model.cuh (the reference's
 // first tutorial: two processes, a buffer, three events); with static_interrupts, workshop_model.cuh's ToolT (test/test_resource.c),
-// cheese_model.cuh (test/test_resourcepool.c) and tutorial2_model.cuh (tutorial/tut_2_1.c); examples/tandem_model.cuh.
+// cheese_model.cuh (test/test_resourcepool.c) and tutorial2_model.cuh (tutorial/tut_2_1.c), and with priority queues and
+// conditions guarded_model.cuh (test/test_objectqueue.c, test/test_priorityqueue.c) and coverage_models.cuh's QueueAndTideT;
+// examples/tandem_model.cuh.
 #pragma once
 
 #include <type_traits>
@@ -136,14 +142,22 @@ struct static_guard {
 // is not a strict weak order (SURVEY.md quirk 1) and the layout decides who is at the top.  At most NPROC entries: a stopped
 // process's entry stays (quirk 2), so only a process restarted while its old entry waits can overflow it (the trial is flagged).
 // Entries are found by key with a scan.
-template <int NPROC>
+struct static_guard_entry {
+    double   d;                 // when the process began to wait
+    uint32_t key;               // the guard sequence number it waits under
+    int32_t  prio;              // its priority then
+    uint32_t subj;
+};
+
+// a cmb_condition's waiter also carries its predicate: m.demand(sim, demand, subj, ctx)
+struct static_condition_entry : static_guard_entry {
+    uint32_t demand;
+    int32_t  ctx;
+};
+
+template <int NPROC, class E = static_guard_entry>
 struct static_heap_guard {
-    struct Entry {
-        double   d;             // when the process began to wait
-        uint32_t key;           // the guard sequence number it waits under
-        int32_t  prio;          // its priority then
-        uint32_t subj;
-    };
+    using Entry = E;
     uint32_t count;
     Entry    e[NPROC + 1];
 
@@ -189,6 +203,15 @@ struct static_heap_guard {
         e[at].key = key;
         e[at].prio = prio;
         e[at].subj = subj;
+        sift_up(at);
+        return true;
+    }
+
+    CMB_FN bool push(const Entry &x)                                   // ... an entry with more than those four fields
+    {
+        if (count >= (uint32_t)NPROC) return false;
+        const uint32_t at = ++count;
+        e[at] = x;
         sift_up(at);
         return true;
     }
@@ -273,6 +296,34 @@ struct static_resource : static_history<RECORD> {
     uint32_t holder;            // process index, NIL = free
 };
 
+// struct cmb_priorityqueue (src/cmb_priorityqueue.c) for a fixed set of processes: at most STATIC_PQ_CAP objects, in a table
+// in the thread's local memory like the guard heaps.  Its order (PrioOrder: priority descending, then handle ascending) is a
+// strict total order, so the first entry of the unsorted table under it is exactly the one the reference's heap gives up next,
+// and no heap layout needs keeping.  A put that finds the table full while `capacity` has room flags the trial (no HBM spill).
+constexpr int STATIC_PQ_CAP = 16;
+
+struct static_pq_entry {
+    uint64_t obj;
+    uint64_t handle;            // the key cmb_priorityqueue_put hands out: 1, 2, ... per queue (HashHeap::issued)
+    int32_t  prio;
+};
+
+template <int NPROC, bool RECORD = false, bool PRE = false>
+struct static_priorityqueue : static_history<RECORD> {
+    static_guard_of<NPROC, PRE> front, rear;
+    static_pq_entry e[STATIC_PQ_CAP];
+    uint64_t capacity;
+    uint64_t issued;
+    uint32_t count;
+};
+
+// struct cmb_condition (src/cmb_condition.c) for a fixed set of processes: its wait list is always the literal heap, in both
+// forms of the tier, because cmb_condition_signal goes over it in array order and that order decides the wake-ups' keys
+template <int NPROC>
+struct static_condition {
+    static_heap_guard<NPROC, static_condition_entry> guard;
+};
+
 // What StaticSim<..., PRE = true> keeps besides: each process's priority (cmb_process_priority) and the key of its guard entry
 // (cmb_process::guard_key), and cmb_random_flip's cache - per trial, as the general engine has it.  A base class, so that the
 // tier's first form (PRE = false) keeps its layout.
@@ -299,9 +350,14 @@ struct StaticSim : StaticPriorities<NPROC, PRE> {
     using recorded_resourcepool_type = static_resourcepool<NPROC, true, PRE>;
     using resource_type = static_resource<NPROC, false, PRE>;
     using recorded_resource_type = static_resource<NPROC, true, PRE>;
+    using priorityqueue_type = static_priorityqueue<NPROC, false, PRE>;
+    using recorded_priorityqueue_type = static_priorityqueue<NPROC, true, PRE>;
+    using condition_type = static_condition<NPROC>;
     using guard_type = static_guard_of<NPROC, PRE>;
+    using condition_guard = static_heap_guard<NPROC, static_condition_entry>;
     static constexpr int PROCESSES = NPROC;
     static constexpr int SLOTS = NPROC + NEVENT;
+    static constexpr bool INTERRUPTS = PRE;
     static_assert(NPROC >= 1 && NPROC <= 32, "a guard's wait list is a 32-bit mask of processes");
     static_assert(!PRE || NEVENT > 0, "interrupts and pre-emptions take spare event slots, and the event list must order by priority");
     static constexpr uint32_t HOLD_BITS = NPROC <= 8 ? 4u : (NPROC <= 16 ? 2u : 1u);
@@ -564,6 +620,71 @@ struct StaticSim : StaticPriorities<NPROC, PRE> {
         g.pop();
         if (!fel.schedule((int)head, ACT_WAKE_RESOURCE, now, prio_of(head))) status |= TRIAL_ERR_FEL_OVERFLOW;
     }
+
+    // cmb_condition_wait up to its yield (src/cmb_condition.c:63-80): the waiter and its predicate go into the condition's heap,
+    // in either form
+    CMB_FN void guard_wait_cmd(condition_guard &g, uint32_t pid, uint32_t demand, int32_t ctx)
+    {
+        const uint32_t s = ++guard_seq;
+        if constexpr (PRE) {
+#pragma unroll
+            for (int i = 0; i < NPROC; i++) {
+                if ((uint32_t)i == pid) this->gkey[i] = s;
+            }
+        }
+        static_condition_entry x;
+        x.d = now;
+        x.key = s;
+        x.prio = prio_of(pid);
+        x.subj = pid;
+        x.demand = demand;
+        x.ctx = ctx;
+        if (!g.push(x)) status |= TRIAL_ERR_GUARD_OVERFLOW;
+        cmd = CMD_NONE;
+    }
+
+    // ... woken by anything but the signal (only an interrupt can, so only in the second form), the waiter takes its entry out
+    CMB_FN int64_t guard_wait_end(condition_guard &g, uint32_t pid, int64_t sig)
+    {
+        if (sig != CMB_PROCESS_SUCCESS) {
+            if constexpr (PRE) {
+                uint32_t key = 0u;
+#pragma unroll
+                for (int i = 0; i < NPROC; i++) {
+                    if ((uint32_t)i == pid) key = this->gkey[i];
+                }
+                g.remove(key);
+            }
+            else {
+                status |= TRIAL_ERR_PROC_OVERFLOW;
+            }
+        }
+        return sig;
+    }
+};
+
+// cmb::Sim::fel_high - the deepest the event list was when an event was taken (cmb_device.cuh's execute) - for a model that says
+// `static constexpr bool static_fel_high = true;` (it reports it).  A class of its own around the tier's StaticSim, so that models
+// without the trait keep their layout; the free functions below take it as the StaticSim it is.
+template <class Base>
+struct StaticSimHigh : Base {
+    uint32_t fel_high;
+
+    template <class... A>
+    CMB_FN void init(A... a)
+    {
+        Base::init(a...);
+        fel_high = 0u;
+    }
+};
+
+template <class Model, class = void>
+struct StaticFelHigh {
+    static constexpr bool value = false;
+};
+template <class Model>
+struct StaticFelHigh<Model, typename std::enable_if<Model::static_fel_high>::type> {
+    static constexpr bool value = true;
 };
 
 // cmb_random_exponential / cmb_random_normal in a process body: inline (a call would take the generator's address and put the
@@ -1114,6 +1235,186 @@ CMB_FN void process_priority_set(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, uin
     }
 }
 
+// cmb_process_priority (0 in the tier's first form)
+template <int NPROC, int NQUEUE, int NEVENT, bool PRE>
+CMB_FN int64_t process_priority(const StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, uint32_t pid)
+{
+    return (int64_t)sim.prio_of(pid);
+}
+
+// ------------------------------------------------------------------------------------------------ priorityqueue
+// as cmb_device.cuh's functions of the same names (src/cmb_priorityqueue.c), over the table
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD, bool PRE>
+CMB_FN void priorityqueue_initialize(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &, static_priorityqueue<NPROC, RECORD, PRE> &q, uint64_t capacity)
+{
+    if constexpr (PRE) {
+        q.front.count = q.rear.count = 0u;
+    }
+    else {
+        q.front.waiting = q.rear.waiting = 0u;
+#pragma unroll
+        for (int i = 0; i < NPROC; i++) q.front.seq[i] = q.rear.seq[i] = 0u;
+    }
+    q.capacity = capacity;
+    q.issued = 0u;
+    q.count = 0u;
+    if constexpr (RECORD) q.recording = 0u;
+}
+
+template <int NPROC, bool RECORD, bool PRE>
+CMB_FN uint64_t priorityqueue_length(const static_priorityqueue<NPROC, RECORD, PRE> &q)
+{
+    return (uint64_t)q.count;
+}
+
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD, bool PRE>
+CMB_FN void priorityqueue_sample(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, static_priorityqueue<NPROC, RECORD, PRE> &q)
+{
+    if constexpr (RECORD) {
+        if (q.recording) q.history.sample((double)q.count, sim.now);
+    }
+}
+
+template <int NPROC, int NQUEUE, int NEVENT, bool PRE>
+CMB_FN void priorityqueue_recording_start(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, static_priorityqueue<NPROC, true, PRE> &q)
+{
+    q.recording = 1u;
+    q.history.start();
+    q.history.sample((double)q.count, sim.now);
+}
+
+template <int NPROC, int NQUEUE, int NEVENT, bool PRE>
+CMB_FN void priorityqueue_recording_stop(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, static_priorityqueue<NPROC, true, PRE> &q)
+{
+    priorityqueue_sample(sim, q);
+    q.recording = 0u;
+}
+
+// PrioOrder (src/cmb_priorityqueue.c:43-54): a strict total order, handles being unique
+CMB_FN bool static_pq_before(const static_pq_entry &a, const static_pq_entry &b)
+{
+    if (a.prio != b.prio) return a.prio > b.prio;
+    return a.handle < b.handle;
+}
+
+// the table index of `handle`, -1 if it is not in the queue
+template <int NPROC, bool RECORD, bool PRE>
+CMB_FN int static_pq_find(const static_priorityqueue<NPROC, RECORD, PRE> &q, uint64_t handle)
+{
+    int at = -1;
+    for (uint32_t k = 0u; k < q.count; k++) {
+        if (q.e[k].handle == handle) at = (int)k;
+    }
+    return at;
+}
+
+// the entry at `at` leaves; the last one takes its place (the table is unsorted)
+template <int NPROC, bool RECORD, bool PRE>
+CMB_FN void static_pq_take(static_priorityqueue<NPROC, RECORD, PRE> &q, int at)
+{
+    q.count--;
+    q.e[at] = q.e[q.count];
+}
+
+template <class Model, int NPROC, int NQUEUE, int NEVENT, bool RECORD, bool PRE>
+CMB_FN bool priorityqueue_try_put(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Model &, static_priorityqueue<NPROC, RECORD, PRE> &q,
+                                  uint64_t obj, int64_t prio, uint64_t *handle)   // :237-284
+{
+    if ((uint64_t)q.count >= q.capacity) return false;
+    const uint64_t h = ++q.issued;
+    if (q.count >= (uint32_t)STATIC_PQ_CAP) {
+        sim.status |= TRIAL_ERR_QUEUE_OVERFLOW;         // void from here on: re-run
+    }
+    else {
+        q.e[q.count].obj = obj;
+        q.e[q.count].handle = h;
+        q.e[q.count].prio = (int32_t)prio;
+        q.count++;
+    }
+    if (handle != nullptr) *handle = h;
+    priorityqueue_sample(sim, q);
+    sim.guard_signal(q.front, true);
+    return true;
+}
+
+template <class Model, int NPROC, int NQUEUE, int NEVENT, bool RECORD, bool PRE>
+CMB_FN bool priorityqueue_try_get(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Model &, static_priorityqueue<NPROC, RECORD, PRE> &q,
+                                  uint64_t &obj)                                  // :189-235
+{
+    if (q.count == 0u) return false;
+    int best = 0;
+    for (uint32_t k = 1u; k < q.count; k++) {
+        if (static_pq_before(q.e[k], q.e[best])) best = (int)k;
+    }
+    obj = q.e[best].obj;
+    static_pq_take(q, best);
+    priorityqueue_sample(sim, q);
+    sim.guard_signal(q.rear, true);
+    return true;
+}
+
+// cmb_priorityqueue_position, :286-320: 1 = next to be taken, 0 = not in the queue
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD, bool PRE>
+CMB_FN uint64_t priorityqueue_position(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &, static_priorityqueue<NPROC, RECORD, PRE> &q, uint64_t handle)
+{
+    const int at = static_pq_find(q, handle);
+    if (at < 0) return 0u;
+    uint64_t ahead = 0u;
+    for (uint32_t k = 0u; k < q.count; k++) {
+        if (static_pq_before(q.e[k], q.e[at])) ahead++;
+    }
+    return ahead + 1u;
+}
+
+// cmb_priorityqueue_cancel: the object leaves without a signal or a history sample, as on the general engine
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD, bool PRE>
+CMB_FN bool priorityqueue_cancel(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &, static_priorityqueue<NPROC, RECORD, PRE> &q, uint64_t handle)
+{
+    const int at = static_pq_find(q, handle);
+    if (at < 0) return false;
+    static_pq_take(q, at);
+    return true;
+}
+
+// cmb_priorityqueue_reprioritize, include/cmb_priorityqueue.h:170-180: the object and its handle stay
+template <int NPROC, int NQUEUE, int NEVENT, bool RECORD, bool PRE>
+CMB_FN void priorityqueue_reprioritize(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &, static_priorityqueue<NPROC, RECORD, PRE> &q, uint64_t handle,
+                                       int64_t prio)
+{
+    const int at = static_pq_find(q, handle);
+    if (at >= 0) q.e[at].prio = (int32_t)prio;
+}
+
+// ------------------------------------------------------------------------------------------------ condition
+template <int NPROC, int NQUEUE, int NEVENT, bool PRE>
+CMB_FN void condition_initialize(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &, static_condition<NPROC> &c)
+{
+    c.guard.count = 0u;
+}
+
+// cmb_condition_signal, src/cmb_condition.c:120-167, as cmb_device.cuh's: every waiter whose predicate holds, in heap-array
+// order, is woken at `now` with its process's priority; the hits leave the heap in a second pass, in the order they were found.
+// The wake-up goes into the waiter's own event slot - empty while it waits - as ACT_WAKE_RESOURCE, which resumes a running
+// process with CMB_PROCESS_SUCCESS exactly as ACT_CMB_WAKE_CONDITION does: no spare slot is needed, and an interrupt that pops
+// first drops it with the rest of the process's slot (cancel_awaiteds), as the general engine's pattern cancel does.
+template <class Model, class S, int NPROC>
+CMB_FN uint32_t condition_signal(S &sim, Model &m, static_condition<NPROC> &c)
+{
+    auto &h = c.guard;
+    if (h.count == 0u) return 0u;
+    uint32_t hit[NPROC];
+    uint32_t n = 0u;
+    for (uint32_t k = 1u; k <= h.count; k++) {
+        const uint32_t pid = h.e[k].subj;
+        if (m.demand(sim, h.e[k].demand, pid, h.e[k].ctx)) {
+            hit[n++] = h.e[k].key;
+            if (!sim.fel.schedule((int)pid, ACT_WAKE_RESOURCE, sim.now, sim.prio_of(pid))) sim.status |= TRIAL_ERR_FEL_OVERFLOW;
+        }
+    }
+    for (uint32_t k = 0u; k < n; k++) h.remove(hit[k]);
+    return n;
+}
+
 // ------------------------------------------------------------------------------------------------ process end
 // A model of the tier's second form may name the pools and resources its processes can hold from:
 //   template <class F> CMB_FN void static_holdables(F &&visit) { visit(cheese); }
@@ -1230,26 +1531,35 @@ struct StaticKinds<Model, decltype((void)Model::static_kind(0u))> {
     }
 };
 
-template <class Model, int NPROC, int NQUEUE, int NEVENT, bool PRE, int I>
+// S: the StaticSim the model was instantiated over (StaticSimHigh<StaticSim<...>> for a model with static_fel_high)
+template <class Model, class S, int I, int NPROC = S::PROCESSES>
 struct StaticDispatch {
-    static CMB_FN void run(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Model &m, int who, int64_t sig)
+    static CMB_FN void run(S &sim, Model &m, int who, int64_t sig)
     {
         if (who == I) m.process(sim, (uint32_t)I, StaticKinds<Model>::template of<I>(sim.proc[I].kind), sig);
-        else StaticDispatch<Model, NPROC, NQUEUE, NEVENT, PRE, I + 1>::run(sim, m, who, sig);
+        else StaticDispatch<Model, S, I + 1>::run(sim, m, who, sig);
     }
 };
-template <class Model, int NPROC, int NQUEUE, int NEVENT, bool PRE>
-struct StaticDispatch<Model, NPROC, NQUEUE, NEVENT, PRE, NPROC> {
-    static CMB_FN void run(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &, Model &, int, int64_t) {}
+template <class Model, class S, int NPROC>
+struct StaticDispatch<Model, S, NPROC, NPROC> {
+    static CMB_FN void run(S &, Model &, int, int64_t) {}
 };
 
 // one step of cmb_event_queue_execute (src/cmb_event.c:229-252): pop, advance the clock, resume the process.  false = the
 // list ran dry.  The body's blocking call is left in sim.cmd for the caller (`who` = the process it belongs to).
-template <class Model, int NPROC, int NQUEUE, int NEVENT, bool PRE>
-CMB_FN bool static_step(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Model &m, int &who)
+template <class Model, class S>
+CMB_FN bool static_step(S &sim, Model &m, int &who)
 {
+    constexpr int NPROC = S::PROCESSES, NEVENT = S::SLOTS - S::PROCESSES;
+    constexpr bool PRE = S::INTERRUPTS;
     uint32_t act, key;
     double when;
+    if constexpr (StaticFelHigh<Model>::value) {
+        uint32_t depth = 0u;
+#pragma unroll
+        for (int i = 0; i < S::SLOTS; i++) depth += sim.fel.key[i] != 0u ? 1u : 0u;
+        if (depth > sim.fel_high) sim.fel_high = depth;
+    }
     if (!sim.fel.pop(who, act, when, key)) return false;
     sim.now = when;
     sim.current_event = key;
@@ -1286,7 +1596,7 @@ CMB_FN bool static_step(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Model &m, in
             who = (int)subj;
             if (run) {
                 sim.current = subj;
-                StaticDispatch<Model, NPROC, NQUEUE, NEVENT, PRE, 0>::run(sim, m, who, arg);
+                StaticDispatch<Model, S, 0>::run(sim, m, who, arg);
                 sim.current = NIL;
             }
             return true;
@@ -1312,7 +1622,7 @@ CMB_FN bool static_step(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Model &m, in
     }
     if (run) {
         sim.current = (uint32_t)who;
-        StaticDispatch<Model, NPROC, NQUEUE, NEVENT, PRE, 0>::run(sim, m, who, CMB_PROCESS_SUCCESS);
+        StaticDispatch<Model, S, 0>::run(sim, m, who, CMB_PROCESS_SUCCESS);
         sim.current = NIL;
     }
     return true;
@@ -1368,12 +1678,17 @@ struct StaticInterrupts<Model, typename std::enable_if<Model::static_interrupts>
     static constexpr bool value = true;
 };
 template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT>
-using StaticSimOf = StaticSim<NPROC, NQUEUE, NEVENT, StaticInterrupts<ModelT<StaticSim<NPROC, NQUEUE, NEVENT>>>::value>;
+using StaticFormOf = StaticSim<NPROC, NQUEUE, NEVENT, StaticInterrupts<ModelT<StaticSim<NPROC, NQUEUE, NEVENT>>>::value>;
+// ... and with `static constexpr bool static_fel_high = true;` it also keeps fel_high (StaticSimHigh)
+template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT>
+using StaticSimOf = typename std::conditional<StaticFelHigh<ModelT<StaticSim<NPROC, NQUEUE, NEVENT>>>::value,
+                                              StaticSimHigh<StaticFormOf<ModelT, NPROC, NQUEUE, NEVENT>>,
+                                              StaticFormOf<ModelT, NPROC, NQUEUE, NEVENT>>::type;
 
 #ifdef CMB_HOST_BUILD
 // the tier's source text run on the CPU (tests/cmb_engine_host.cpp): one trial, the slow path taken where it occurs
-template <class Model, int NPROC, int NQUEUE, int NEVENT, bool PRE>
-inline void static_run_trial_host(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Model &m, const TrialIn &in, TrialOut &out,
+template <class Model, class S>
+inline void static_run_trial_host(S &sim, Model &m, const TrialIn &in, TrialOut &out,
                                   uint64_t trace_cap, uint64_t *trace_key, double *trace_time)
 {
     out.objects = 0u;
@@ -1399,12 +1714,12 @@ inline void static_run_trial_host(StaticSim<NPROC, NQUEUE, NEVENT, PRE> &sim, Mo
             const Sfc64 saved = sim.rng;
             sim.hot_only = true;
             sim.hot_failed = false;
-            double dur = ModelSampler<Model, StaticSim<NPROC, NQUEUE, NEVENT, PRE>>::draw(m, sim, sim.cmd_sample);
+            double dur = ModelSampler<Model, S>::draw(m, sim, sim.cmd_sample);
             sim.hot_only = false;
             if (sim.hot_failed) {
                 sim.hot_failed = false;
                 sim.rng = saved;
-                dur = ModelSampler<Model, StaticSim<NPROC, NQUEUE, NEVENT, PRE>>::draw(m, sim, sim.cmd_sample);
+                dur = ModelSampler<Model, S>::draw(m, sim, sim.cmd_sample);
             }
             if (dur < 0.0) sim.status |= TRIAL_ERR_NEGATIVE_HOLD;
             if (!sim.fel.schedule(who, ACT_WAKE_TIME, __dadd_rn(sim.now, dur), sim.prio_of((uint32_t)who))) sim.status |= TRIAL_ERR_FEL_OVERFLOW;

@@ -9,6 +9,7 @@
 //                 guard OBSERVES a resource's guard
 #pragma once
 #include "../csrc/cmb_kernel.cuh"
+#include "../csrc/cmb_static.cuh"
 
 namespace cimba_b200 {
 namespace models {
@@ -134,9 +135,13 @@ struct PoolFight {
     }
 };
 
-struct QueueAndTide {
-    cmb::priorityqueue pq;
-    cmb::condition     tide_cv;
+// A template over the engine: QueueAndTideT<cmb::Sim> is the general-engine model (QueueAndTide); on the static tier it runs in the
+// second form with 8 processes and 2 spare event slots (the end event and the nuisance's interrupt), its priority queue in the
+// tier's table and the condition's wake-ups in the waiters' own slots.
+template <class S>
+struct QueueAndTideT {
+    typename S::priorityqueue_type pq;
+    typename S::condition_type     tide_cv;
     uint64_t counter[8];
     uint64_t last_handle[2];
     double   sum_wait, put_mean, get_mean;
@@ -145,6 +150,12 @@ struct QueueAndTide {
     enum : uint32_t { END_EVENT = cmb::ACT_CMB_USER };
     enum : uint32_t { HIGH_ENOUGH = 100u };
     static constexpr uint32_t PROCS = 7u;
+    static constexpr bool static_interrupts = true;
+    static constexpr bool static_fel_high = true;
+    static CMB_FN constexpr uint32_t static_kind(uint32_t i)
+    {
+        return i < 2u ? PRODUCER : i == 2u ? CONSUMER : i == 3u ? SHUFFLER : i == 4u ? TIDE : i < PROCS ? WAITER : NUISANCE;
+    }
 
     CMB_FN void note(int64_t sig)
     {
@@ -152,9 +163,9 @@ struct QueueAndTide {
     }
 
     // u[0] = weight, u[1] = handle, fr... the priority of the put lives in proc.f[0] (as an integer value)
-    CMB_FN void producer(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void producer(S &sim, uint32_t me, int64_t sig)
     {
-        QueueAndTide &m = *this;
+        QueueAndTideT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(put_mean);
@@ -175,9 +186,9 @@ struct QueueAndTide {
         CMB_PROCESS_END
     }
 
-    CMB_FN void consumer(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void consumer(S &sim, uint32_t me, int64_t sig)
     {
-        QueueAndTide &m = *this;
+        QueueAndTideT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(get_mean);
@@ -195,9 +206,9 @@ struct QueueAndTide {
         CMB_PROCESS_END
     }
 
-    CMB_FN void shuffler(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void shuffler(S &sim, uint32_t me, int64_t sig)
     {
-        QueueAndTide &m = *this;
+        QueueAndTideT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(1.5);
@@ -222,9 +233,9 @@ struct QueueAndTide {
         CMB_PROCESS_END
     }
 
-    CMB_FN void tide(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void tide(S &sim, uint32_t me, int64_t sig)
     {
-        QueueAndTide &m = *this;
+        QueueAndTideT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(1.0);
@@ -236,9 +247,9 @@ struct QueueAndTide {
     }
 
     // u[0] = "through" flag of the pass in progress
-    CMB_FN void waiter(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void waiter(S &sim, uint32_t me, int64_t sig)
     {
-        QueueAndTide &m = *this;
+        QueueAndTideT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             sim.proc[me].u[0] = 1u;
@@ -257,9 +268,9 @@ struct QueueAndTide {
         CMB_PROCESS_END
     }
 
-    CMB_FN void nuisance(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void nuisance(S &sim, uint32_t me, int64_t sig)
     {
-        QueueAndTide &m = *this;
+        QueueAndTideT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(1.0);
@@ -273,7 +284,7 @@ struct QueueAndTide {
         CMB_PROCESS_END
     }
 
-    CMB_FN void run_trial(cmb::Sim &sim, const cmb::TrialIn &in)
+    CMB_FN void run_trial(S &sim, const cmb::TrialIn &in)
     {
         for (uint32_t i = 0u; i < 8u; i++) counter[i] = 0u;
         sum_wait = 0.0;
@@ -294,7 +305,7 @@ struct QueueAndTide {
         (void)cmb_event_schedule(END_EVENT, cmb::NIL, 0, (double)in.num_objects, 0);
     }
 
-    CMB_FN void process(cmb::Sim &sim, uint32_t me, uint32_t kind, int64_t sig)
+    CMB_FN void process(S &sim, uint32_t me, uint32_t kind, int64_t sig)
     {
         switch (kind) {
         case PRODUCER: producer(sim, me, sig); break;
@@ -306,17 +317,17 @@ struct QueueAndTide {
         }
     }
 
-    CMB_FN void event(cmb::Sim &sim, uint32_t action, uint32_t, int64_t)
+    CMB_FN void event(S &sim, uint32_t action, uint32_t, int64_t)
     {
-        QueueAndTide &m = *this;
+        QueueAndTideT &m = *this;
         if (action == END_EVENT) {
             for (uint32_t i = 0u; i <= PROCS; i++) cmb_process_stop(i, 0);
         }
     }
 
-    CMB_FN bool demand(cmb::Sim &, uint32_t, uint32_t, int32_t ctx) { return level >= threshold[ctx]; }
+    CMB_FN bool demand(S &, uint32_t, uint32_t, int32_t ctx) { return level >= threshold[ctx]; }
 
-    CMB_FN void finish(cmb::Sim &sim, cmb::TrialOut &out)
+    CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         counter[7] = cmb_priorityqueue_length(pq);
         for (uint32_t i = 0u; i < 8u; i++) out.counters[i] = counter[i];
@@ -325,6 +336,8 @@ struct QueueAndTide {
         out.max_queue = sim.fel_high;
     }
 };
+
+using QueueAndTide = QueueAndTideT<cmb::Sim>;
 
 struct FrontDesk {
     cmb::resource  desk;

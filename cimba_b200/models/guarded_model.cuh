@@ -5,21 +5,30 @@
 // test/reference/objectqueue.txt); RECORD = the length history on; PRIORITY = true: a cmb_priorityqueue, objects put with the putter's own priority, history
 // on (model 13, test/reference/priorityqueue.txt).  The object is the time it was put (a double's bits).
 // Oracle: oracle/ref_build/ref_driver.c run_guarded_trial (the counters are described there).
+// A template over the engine: GuardedT<cmb::Sim, P, R> is the general-engine model (Guarded<P, R>), and on the static tier
+// GuardedT<cmb::StaticSimOf<...>> runs in the tier's second form (static_interrupts) with 7 processes and 2 spare event slots -
+// the end event and the nuisance's interrupt, which pops at the time it was made - and a queue window of 32 entries.
 #pragma once
+#include <type_traits>
+
 #include "../csrc/cmb_kernel.cuh"
+#include "../csrc/cmb_static.cuh"
 
 namespace cimba_b200 {
 namespace models {
 
-template <bool PRIORITY, bool RECORD>
-struct Guarded {
-    cmb::objectqueue   queue;
-    cmb::priorityqueue pq;
+template <class S, bool PRIORITY, bool RECORD>
+struct GuardedT {
+    typename std::conditional<RECORD, typename S::recorded_queue_type, typename S::queue_type>::type queue;
+    typename S::recorded_priorityqueue_type pq;
     uint64_t counter[8];
     double   sum_wait, put_mean, get_mean;
     enum : uint32_t { PUTTER, GETTER, NUISANCE };
     enum : uint32_t { END_EVENT = cmb::ACT_CMB_USER };
     static constexpr uint32_t PUTTERS = 3u, GETTERS = 3u, WORKERS = 6u;
+    static constexpr bool static_interrupts = true;
+    static constexpr bool static_fel_high = !PRIORITY && !RECORD;     // model 3 reports it (the others their history's size)
+    static CMB_FN constexpr uint32_t static_kind(uint32_t i) { return i < PUTTERS ? PUTTER : (i < WORKERS ? GETTER : NUISANCE); }
 
     CMB_FN void note_signal(int64_t sig, uint32_t which)
     {
@@ -29,9 +38,9 @@ struct Guarded {
         }
     }
 
-    CMB_FN void putter(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void putter(S &sim, uint32_t me, int64_t sig)
     {
-        Guarded &m = *this;
+        GuardedT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(put_mean);
@@ -45,9 +54,9 @@ struct Guarded {
         CMB_PROCESS_END
     }
 
-    CMB_FN void getter(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void getter(S &sim, uint32_t me, int64_t sig)
     {
-        Guarded &m = *this;
+        GuardedT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(get_mean);
@@ -65,9 +74,9 @@ struct Guarded {
         CMB_PROCESS_END
     }
 
-    CMB_FN void nuisance(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void nuisance(S &sim, uint32_t me, int64_t sig)
     {
-        Guarded &m = *this;
+        GuardedT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(1.0);
@@ -82,19 +91,19 @@ struct Guarded {
         CMB_PROCESS_END
     }
 
-    CMB_FN void run_trial(cmb::Sim &sim, const cmb::TrialIn &in)
+    CMB_FN void run_trial(S &sim, const cmb::TrialIn &in)
     {
         for (uint32_t i = 0u; i < 8u; i++) counter[i] = 0u;
         sum_wait = 0.0;
         put_mean = in.arr_mean;
         get_mean = in.srv_mean;
-        if (PRIORITY) {
+        if constexpr (PRIORITY) {
             cmb_priorityqueue_initialize(pq, (uint64_t)in.servers);
             cmb_priorityqueue_recording_start(pq);
         }
         else {
             cmb_objectqueue_initialize(queue, (uint64_t)in.servers);
-            if (RECORD) cmb_objectqueue_recording_start(queue);
+            if constexpr (RECORD) cmb_objectqueue_recording_start(queue);
         }
         for (uint32_t i = 0u; i < WORKERS; i++) {
             const int64_t pri = cmb_random_dice(-5, 5);
@@ -104,41 +113,51 @@ struct Guarded {
         (void)cmb_event_schedule(END_EVENT, cmb::NIL, 0, (double)in.num_objects, 0);
     }
 
-    CMB_FN void process(cmb::Sim &sim, uint32_t me, uint32_t kind, int64_t sig)
+    CMB_FN void process(S &sim, uint32_t me, uint32_t kind, int64_t sig)
     {
         if (kind == PUTTER) putter(sim, me, sig);
         else if (kind == GETTER) getter(sim, me, sig);
         else nuisance(sim, me, sig);
     }
 
-    CMB_FN void event(cmb::Sim &sim, uint32_t action, uint32_t, int64_t)
+    CMB_FN void event(S &sim, uint32_t action, uint32_t, int64_t)
     {
-        Guarded &m = *this;
+        GuardedT &m = *this;
         if (action == END_EVENT) {
             for (uint32_t i = 0u; i <= WORKERS; i++) cmb_process_stop(i, 0);
         }
     }
-    CMB_FN bool demand(cmb::Sim &, uint32_t, uint32_t, int32_t) { return false; }
+    CMB_FN bool demand(S &, uint32_t, uint32_t, int32_t) { return false; }
 
-    CMB_FN void finish(cmb::Sim &sim, cmb::TrialOut &out)
+    CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         counter[6] = PRIORITY ? cmb_priorityqueue_length(pq) : cmb_objectqueue_length(queue);
-        out.max_queue = sim.fel_high;
-        if (PRIORITY) {
+        if constexpr (PRIORITY) {
             cmb_priorityqueue_recording_stop(pq);
             counter[6] = (uint64_t)__double_as_longlong(pq.history.acc.m1);
             out.max_queue = (uint32_t)pq.history.acc.count;
         }
-        else if (RECORD) {
+        else if constexpr (RECORD) {
             cmb_objectqueue_recording_stop(queue);
             counter[6] = (uint64_t)__double_as_longlong(queue.history.acc.m1);
             out.max_queue = (uint32_t)queue.history.acc.count;
+        }
+        else {
+            out.max_queue = sim.fel_high;
         }
         for (uint32_t i = 0u; i < 8u; i++) out.counters[i] = counter[i];
         out.objects = counter[1];
         out.sum_wait = sum_wait;
     }
 };
+
+template <bool PRIORITY, bool RECORD>
+using Guarded = GuardedT<cmb::Sim, PRIORITY, RECORD>;
+
+// the three as templates over the engine alone, for the static tier's launch
+template <class S> using GuardedQueueT = GuardedT<S, false, false>;             // model 3
+template <class S> using GuardedRecordedQueueT = GuardedT<S, false, true>;      // model 11
+template <class S> using GuardedPriorityQueueT = GuardedT<S, true, true>;       // model 13
 
 }  // namespace models
 }  // namespace cimba_b200

@@ -158,7 +158,9 @@ const char *cimba_b200_model_name(int model_id);
 /* CIMBA_B200_MODEL_MM1 / _GG1 / _MM1_RECORDED from their authoring-surface source on the static tier (cimba_b200/csrc/cmb_static.cuh):
  * process records and event slots in registers, the queue in shared memory; what it flags is re-run on the general engine.
  * Also CIMBA_B200_MODEL_RESOURCE_RECORDED, _POOL_RECORDED and _TUTORIAL2 on the tier's form with priorities, interrupts and
- * pre-emption (same workspace as their default route; the default routes are unchanged) */
+ * pre-emption (same workspace as their default route; the default routes are unchanged), and CIMBA_B200_MODEL_GUARDED,
+ * _GUARDED_RECORDED, _PRIOQ_RECORDED and _PRIOQ with the tier's priority queue and condition (the same workspace as their default
+ * route at every capacity; a queue beyond the tier's tables is re-run on the general engine) */
 #define CIMBA_B200_VARIANT_STATIC 17
 
 /* Error codes */
