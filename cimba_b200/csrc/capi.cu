@@ -704,7 +704,9 @@ const Route *route(const cimba_b200_device_job *job)
     case CIMBA_B200_MODEL_PREEMPT:            return coverage_route<models::PoolFight>(job, INT32_MAX);   // no table sized by `servers`
     case CIMBA_B200_MODEL_BUFFER:             return coverage_route<models::Workshop<false>>(job, INT32_MAX);
     case CIMBA_B200_MODEL_BUFFER_RECORDED:    return coverage_route<models::Workshop<true>>(job, INT32_MAX);
-    case CIMBA_B200_MODEL_TIMERS:             return coverage_route<models::FrontDesk>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_TIMERS:
+        return on_static ? &STATIC_IN<models::FrontDeskT, 8, models::FRONTDESK_SPARE_SLOTS, coverage_workspace, false>
+                         : coverage_route<models::FrontDesk>(job, INT32_MAX);
     case CIMBA_B200_MODEL_RESOURCE_RECORDED:
         return on_static ? &STATIC_IN<models::ToolT, 4, 2, coverage_workspace, false> : coverage_route<models::Tool>(job, INT32_MAX);
     }

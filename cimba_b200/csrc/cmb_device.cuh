@@ -990,6 +990,13 @@ CMB_FN void guard_register(Model &m, resourceguard &g, resourceguard &observer)
     else g.observers[1] = off;
 }
 
+// ... as the authoring surface calls it, with the sim (the static tier, cmb_static.cuh, keeps its observer links there)
+template <class Model>
+CMB_FN void guard_register(Sim &, Model &m, resourceguard &g, resourceguard &observer)
+{
+    guard_register(m, g, observer);
+}
+
 // ------------------------------------------------------------------------------------------------ objectqueue
 CMB_FN void objectqueue_initialize(Sim &sim, objectqueue &q, uint64_t capacity)    // src/cmb_objectqueue.c:54-113
 {
@@ -1803,4 +1810,4 @@ CMB_FN double draw_std_normal(Sim &sim) { return gp_std_normal(sim.rng, *sim.hot
 #define cmb_objectqueue_recording_stop(q)   (cimba_b200::cmb::objectqueue_recording_stop(sim, (q)))
 #define cmb_condition_initialize(c)         (cimba_b200::cmb::condition_initialize(sim, (c)))
 #define cmb_condition_signal(c)             (cimba_b200::cmb::condition_signal(sim, m, (c)))
-#define cmb_resourceguard_register(g, obs)  (cimba_b200::cmb::guard_register(m, (g), (obs)))
+#define cmb_resourceguard_register(g, obs)  (cimba_b200::cmb::guard_register(sim, m, (g), (obs)))

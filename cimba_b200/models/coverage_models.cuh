@@ -339,9 +339,17 @@ struct QueueAndTideT {
 
 using QueueAndTide = QueueAndTideT<cmb::Sim>;
 
-struct FrontDesk {
-    cmb::resource  desk;
-    cmb::condition desk_free;
+// A template over the engine: FrontDeskT<cmb::Sim> is the general-engine model (FrontDesk); on the static tier it runs in the
+// second form with static_waits - 8 processes and FRONTDESK_SPARE_SLOTS spare event slots for the end event, the bells, the
+// patients' timers, the nuisance's interrupt, the clerk's resumes and the wake-ups of waits on the clerk and on the bell.
+// 8 is the most the vector cases of tests/golden/cmb_engine_vectors.json have pending at once: with 7 some of them flag, with 8
+// none.  A trial that needs more is flagged and re-run on the general engine.
+constexpr int FRONTDESK_SPARE_SLOTS = 8;
+
+template <class S>
+struct FrontDeskT {
+    typename S::resource_type  desk;
+    typename S::condition_type desk_free;
     uint64_t counter[8];
     uint64_t bell;
     double   sum_wait, arr_mean, srv_mean;
@@ -351,6 +359,15 @@ struct FrontDesk {
     enum : uint32_t { DESK_IS_FREE = 100u };
     enum : int64_t { SIG_ALARM = 77, SIG_DOZE = 55, SIG_NUDGE = 9 };
     static constexpr uint32_t PROCS = 8u, THE_CLERK = 2u;
+    static constexpr bool static_interrupts = true;
+    static constexpr bool static_waits = true;
+    static constexpr bool static_fel_high = true;
+    static CMB_FN constexpr uint32_t static_kind(uint32_t i)
+    {
+        return i < 2u ? PATIENT : i == 2u ? CLERK : i == 3u ? SUPERVISOR : i == 4u ? RINGER : i == 5u ? LISTENER : i == 6u ? WATCHER : NUISANCE;
+    }
+    template <class F>
+    CMB_FN void static_holdables(F &&visit) { visit(desk); }
 
     CMB_FN void note(int64_t sig)
     {
@@ -358,9 +375,9 @@ struct FrontDesk {
     }
 
     // u[0] = the patience timer's handle, f[0] = when the desk was taken
-    CMB_FN void patient(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void patient(S &sim, uint32_t me, int64_t sig)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(arr_mean);
@@ -394,9 +411,9 @@ struct FrontDesk {
     }
 
     // u[0] = jobs this time, u[1] = jobs done
-    CMB_FN void clerk(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void clerk(S &sim, uint32_t me, int64_t sig)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         CMB_PROCESS_BEGIN
         clerk_start_pending = 0u;
         sim.proc[me].u[0] = (uint64_t)cmb_random_dice(2, 5);
@@ -410,9 +427,9 @@ struct FrontDesk {
         CMB_PROCESS_END
     }
 
-    CMB_FN void supervisor(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void supervisor(S &sim, uint32_t me, int64_t sig)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_WAIT_PROCESS(THE_CLERK);
@@ -433,9 +450,9 @@ struct FrontDesk {
     }
 
     // u[0] = the bell's handle
-    CMB_FN void ringer(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void ringer(S &sim, uint32_t me, int64_t sig)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             sim.proc[me].f[0] = __dadd_rn(cmb_time(), cmb_random_exponential(2.0));
@@ -466,9 +483,9 @@ struct FrontDesk {
         CMB_PROCESS_END
     }
 
-    CMB_FN void listener(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void listener(S &sim, uint32_t me, int64_t sig)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             if (bell != 0u && cmb_event_is_scheduled(bell)) {
@@ -484,9 +501,9 @@ struct FrontDesk {
         CMB_PROCESS_END
     }
 
-    CMB_FN void watcher(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void watcher(S &sim, uint32_t me, int64_t sig)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_CONDITION_WAIT(desk_free, DESK_IS_FREE, 0);
@@ -498,9 +515,9 @@ struct FrontDesk {
         CMB_PROCESS_END
     }
 
-    CMB_FN void nuisance(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void nuisance(S &sim, uint32_t me, int64_t sig)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(1.0);
@@ -514,9 +531,9 @@ struct FrontDesk {
         CMB_PROCESS_END
     }
 
-    CMB_FN void run_trial(cmb::Sim &sim, const cmb::TrialIn &in)
+    CMB_FN void run_trial(S &sim, const cmb::TrialIn &in)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         for (uint32_t i = 0u; i < 8u; i++) counter[i] = 0u;
         sum_wait = 0.0;
         arr_mean = in.arr_mean;
@@ -534,7 +551,7 @@ struct FrontDesk {
         (void)cmb_event_schedule(END_EVENT, cmb::NIL, 0, (double)in.num_objects, 0);
     }
 
-    CMB_FN void process(cmb::Sim &sim, uint32_t me, uint32_t kind, int64_t sig)
+    CMB_FN void process(S &sim, uint32_t me, uint32_t kind, int64_t sig)
     {
         switch (kind) {
         case PATIENT:    patient(sim, me, sig); break;
@@ -547,9 +564,9 @@ struct FrontDesk {
         }
     }
 
-    CMB_FN void event(cmb::Sim &sim, uint32_t action, uint32_t, int64_t)
+    CMB_FN void event(S &sim, uint32_t action, uint32_t, int64_t)
     {
-        FrontDesk &m = *this;
+        FrontDeskT &m = *this;
         if (action == BELL_EVENT) {
             counter[4] += 1u;
         }
@@ -560,9 +577,9 @@ struct FrontDesk {
         }
     }
 
-    CMB_FN bool demand(cmb::Sim &, uint32_t, uint32_t, int32_t) { return desk.holder == cmb::NIL; }
+    CMB_FN bool demand(S &, uint32_t, uint32_t, int32_t) { return desk.holder == cmb::NIL; }
 
-    CMB_FN void finish(cmb::Sim &sim, cmb::TrialOut &out)
+    CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         for (uint32_t i = 0u; i < 8u; i++) out.counters[i] = counter[i];
         out.objects = counter[0];
@@ -570,6 +587,8 @@ struct FrontDesk {
         out.max_queue = sim.fel_high;
     }
 };
+
+using FrontDesk = FrontDeskT<cmb::Sim>;
 
 }  // namespace models
 }  // namespace cimba_b200

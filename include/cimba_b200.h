@@ -160,7 +160,9 @@ const char *cimba_b200_model_name(int model_id);
  * Also CIMBA_B200_MODEL_RESOURCE_RECORDED, _POOL_RECORDED and _TUTORIAL2 on the tier's form with priorities, interrupts and
  * pre-emption (same workspace as their default route; the default routes are unchanged), and CIMBA_B200_MODEL_GUARDED,
  * _GUARDED_RECORDED, _PRIOQ_RECORDED and _PRIOQ with the tier's priority queue and condition (the same workspace as their default
- * route at every capacity; a queue beyond the tier's tables is re-run on the general engine) */
+ * route at every capacity; a queue beyond the tier's tables is re-run on the general engine), and CIMBA_B200_MODEL_TIMERS with the
+ * tier's timers, resume / yield, waits on processes and events and observers (same workspace as its default route; a trial that
+ * needs a ninth spare event slot, or cancels a waited-on event in an order the tier does not keep, is re-run on the general engine) */
 #define CIMBA_B200_VARIANT_STATIC 17
 
 /* Error codes */
