@@ -701,9 +701,15 @@ const Route *route(const cimba_b200_device_job *job)
         return on_static ? &STATIC_COVERAGE<models::GuardedPriorityQueueT, 7, 0, 2, 15> : coverage_route<models::Guarded<true, true>>(job, 15);
     case CIMBA_B200_MODEL_PRIOQ:
         return on_static ? &STATIC_COVERAGE<models::QueueAndTideT, 8, 0, 2, 15> : coverage_route<models::QueueAndTide>(job, 15);
-    case CIMBA_B200_MODEL_PREEMPT:            return coverage_route<models::PoolFight>(job, INT32_MAX);   // no table sized by `servers`
-    case CIMBA_B200_MODEL_BUFFER:             return coverage_route<models::Workshop<false>>(job, INT32_MAX);
-    case CIMBA_B200_MODEL_BUFFER_RECORDED:    return coverage_route<models::Workshop<true>>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_PREEMPT:            // no table sized by `servers`
+        return on_static ? &STATIC_IN<models::PoolFightT, 6, models::POOLFIGHT_SPARE_SLOTS, coverage_workspace, true>
+                         : coverage_route<models::PoolFight>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_BUFFER:
+        return on_static ? &STATIC_IN<models::WorkshopBufferT, 7, models::WORKSHOP_SPARE_SLOTS, coverage_workspace, true>
+                         : coverage_route<models::Workshop<false>>(job, INT32_MAX);
+    case CIMBA_B200_MODEL_BUFFER_RECORDED:
+        return on_static ? &STATIC_IN<models::WorkshopRecordedT, 7, models::WORKSHOP_SPARE_SLOTS, coverage_workspace, true>
+                         : coverage_route<models::Workshop<true>>(job, INT32_MAX);
     case CIMBA_B200_MODEL_TIMERS:
         return on_static ? &STATIC_IN<models::FrontDeskT, 8, models::FRONTDESK_SPARE_SLOTS, coverage_workspace, false>
                          : coverage_route<models::FrontDesk>(job, INT32_MAX);

@@ -40,10 +40,12 @@
 // A model is `template <class S> struct M` with S = cmb::Sim or cmb::StaticSim<...>, its queues declared as
 // `typename S::queue_type`, exported with CMB_EXPORT_STATIC_MODEL(M, NPROC, NQUEUE, "name") (or ..._EVENTS(M, NPROC, NQUEUE,
 // NEVENT, "name")).  In this library: mm1_model.cuh, gg1_model.cuh, mm1_recorded_model.cuh, tutorial1_model.cuh (the reference's
-// first tutorial: two processes, a buffer, three events); with static_interrupts, workshop_model.cuh's ToolT (test/test_resource.c),
-// cheese_model.cuh (test/test_resourcepool.c) and tutorial2_model.cuh (tutorial/tut_2_1.c), and with priority queues and
-// conditions guarded_model.cuh (test/test_objectqueue.c, test/test_priorityqueue.c) and coverage_models.cuh's QueueAndTideT;
-// with static_waits coverage_models.cuh's FrontDeskT; examples/tandem_model.cuh.
+// first tutorial: two processes, a buffer, three events); with static_interrupts, workshop_model.cuh's ToolT (test/test_resource.c)
+// and WorkshopT (test/test_buffer.c and the buffer-and-resource world: the buffer in the second form), cheese_model.cuh
+// (test/test_resourcepool.c), coverage_models.cuh's PoolFightT (test/test_resourcepool.c's cast with checks) and
+// tutorial2_model.cuh (tutorial/tut_2_1.c), and with priority queues and conditions guarded_model.cuh (test/test_objectqueue.c,
+// test/test_priorityqueue.c) and coverage_models.cuh's QueueAndTideT; with static_waits coverage_models.cuh's FrontDeskT;
+// examples/tandem_model.cuh.
 #pragma once
 
 #include <type_traits>
@@ -2085,6 +2087,19 @@ struct StaticLookahead<Model, typename std::enable_if<Model::exponential_holds_o
     static constexpr bool value = true;
 };
 
+// The kernel's launch bounds give ptxas 64 threads per CTA and, by default, no minimum of CTAs per SM: ptxas then picks a register
+// target of its own, and for some models (coverage_models.cuh's PoolFightT, workshop_model.cuh's WorkshopT) that target is below
+// what the step needs and it spills.  Such a model says `static constexpr int static_min_ctas = 1;`: one CTA per SM bounds the
+// registers at 255 only, and ptxas allocates what the code needs.  0 (the default) leaves the bounds as they were.
+template <class Model, class = void>
+struct StaticMinCtas {
+    static constexpr int value = 0;
+};
+template <class Model>
+struct StaticMinCtas<Model, typename std::enable_if<(Model::static_min_ctas > 0)>::type> {
+    static constexpr int value = Model::static_min_ctas;
+};
+
 struct StaticArgs {
     LaunchArgs base;
     double    *spill;           // [num_trials][NQUEUE][spill_cap]
@@ -2092,7 +2107,7 @@ struct StaticArgs {
 };
 
 template <template <class> class ModelT, int NPROC, int NQUEUE, int NEVENT, bool TRACE>
-__global__ void __launch_bounds__(STATIC_BLOCK)
+__global__ void __launch_bounds__(STATIC_BLOCK, StaticMinCtas<ModelT<StaticSim<NPROC, NQUEUE, NEVENT>>>::value)
 static_trial_kernel(const StaticArgs sa)
 {
     using S = StaticSimOf<ModelT, NPROC, NQUEUE, NEVENT>;

@@ -1,12 +1,14 @@
 // coverage_models.cuh - the three "everything at once" workloads of the parity suite written against the authoring surface
 // (the same worlds the reference runs in oracle/ref_build/ref_driver.c, where the counters are described):
-//   PoolFight     (model 4) test/test_resourcepool.c's cast with checks: mice changing their own priority and acquiring, rats
+//   PoolFightT    (model 4) test/test_resourcepool.c's cast with checks: mice changing their own priority and acquiring, rats
 //                 pre-empting, a cat interrupting, partial releases, cmb_resourcepool_held_by_process compared with the body's own count
-//   QueueAndTide  (model 6) cmb_priorityqueue put / get / position / cancel / reprioritize by handle + cmb_condition with two
+//   QueueAndTideT (model 6) cmb_priorityqueue put / get / position / cancel / reprioritize by handle + cmb_condition with two
 //                 predicates, under a nuisance
-//   FrontDesk     (model 8) timers (add / cancel / set / clear), cmb_process_yield + resume, wait_process on a process that exits
+//   FrontDeskT    (model 8) timers (add / cancel / set / clear), cmb_process_yield + resume, wait_process on a process that exits
 //                 and is started again, wait_event on events that get rescheduled / reprioritized / cancelled, a condition whose
 //                 guard OBSERVES a resource's guard
+// Each is a template over the engine (cmb::Sim, or the static tier's second form); PoolFight, QueueAndTide and FrontDesk name their
+// general-engine forms.
 #pragma once
 #include "../csrc/cmb_kernel.cuh"
 #include "../csrc/cmb_static.cuh"
@@ -14,20 +16,34 @@
 namespace cimba_b200 {
 namespace models {
 
-struct PoolFight {
-    cmb::resourcepool pool;
+// A template over the engine: PoolFightT<cmb::Sim> is the general-engine model (PoolFight); on the static tier it runs in the
+// second form with 6 processes and POOLFIGHT_SPARE_SLOTS spare event slots for the end event, the cat's interrupt and a rat's
+// pre-emption, which interrupts every victim at once.  4 is the fewest at which no vector case of
+// tests/golden/cmb_engine_vectors.json flags (with 3, half of them do); a trial that needs more is flagged and re-run on the general
+// engine - about 1.9 % of them at capacity 10 and 500 time units.
+constexpr int POOLFIGHT_SPARE_SLOTS = 4;
+
+template <class S>
+struct PoolFightT {
+    typename S::resourcepool_type pool;
     uint64_t counter[8];
     double   sum_wait;
     enum : uint32_t { MOUSE, RAT, CAT };
     enum : uint32_t { END_EVENT = cmb::ACT_CMB_USER };
     static constexpr uint32_t MICE = 3u, RODENTS = 5u;
+    static constexpr bool static_interrupts = true;
+    static constexpr bool static_fel_high = true;
+    static constexpr int static_min_ctas = 1;       // without it ptxas holds the kernel to 128 registers and spills
+    static CMB_FN constexpr uint32_t static_kind(uint32_t i) { return i < MICE ? MOUSE : i < RODENTS ? RAT : CAT; }
+    template <class F>
+    CMB_FN void static_holdables(F &&visit) { visit(pool); }
 
-    CMB_FN void check(cmb::Sim &sim, uint32_t me)
+    CMB_FN void check(S &sim, uint32_t me)
     {
         if (cmb_resourcepool_held_by_process(pool, me) != sim.proc[me].u[0]) counter[7] += 1u;
     }
 
-    CMB_FN void signal(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void signal(S &sim, uint32_t me, int64_t sig)
     {
         if (sig == CMB_PROCESS_PREEMPTED) {
             counter[2] += 1u;
@@ -40,9 +56,9 @@ struct PoolFight {
     }
 
     // u[0] = units held by the body's own count, u[1] = the request in progress
-    CMB_FN void rodent(cmb::Sim &sim, uint32_t me, int64_t sig, bool rat)
+    CMB_FN void rodent(S &sim, uint32_t me, int64_t sig, bool rat)
     {
-        PoolFight &m = *this;
+        PoolFightT &m = *this;
         CMB_PROCESS_BEGIN
         sim.proc[me].u[0] = 0u;
         for (;;) {
@@ -82,9 +98,9 @@ struct PoolFight {
         CMB_PROCESS_END
     }
 
-    CMB_FN void cat(cmb::Sim &sim, uint32_t me, int64_t sig)
+    CMB_FN void cat(S &sim, uint32_t me, int64_t sig)
     {
-        PoolFight &m = *this;
+        PoolFightT &m = *this;
         CMB_PROCESS_BEGIN
         for (;;) {
             CMB_PROCESS_HOLD_EXPONENTIAL(1.0);
@@ -97,7 +113,7 @@ struct PoolFight {
         CMB_PROCESS_END
     }
 
-    CMB_FN void run_trial(cmb::Sim &sim, const cmb::TrialIn &in)
+    CMB_FN void run_trial(S &sim, const cmb::TrialIn &in)
     {
         for (uint32_t i = 0u; i < 8u; i++) counter[i] = 0u;
         sum_wait = 0.0;
@@ -110,22 +126,22 @@ struct PoolFight {
         (void)cmb_event_schedule(END_EVENT, cmb::NIL, 0, (double)in.num_objects, 0);
     }
 
-    CMB_FN void process(cmb::Sim &sim, uint32_t me, uint32_t kind, int64_t sig)
+    CMB_FN void process(S &sim, uint32_t me, uint32_t kind, int64_t sig)
     {
         if (kind == CAT) cat(sim, me, sig);
         else rodent(sim, me, sig, kind == RAT);
     }
 
-    CMB_FN void event(cmb::Sim &sim, uint32_t action, uint32_t, int64_t)
+    CMB_FN void event(S &sim, uint32_t action, uint32_t, int64_t)
     {
-        PoolFight &m = *this;
+        PoolFightT &m = *this;
         if (action == END_EVENT) {
             for (uint32_t i = 0u; i <= RODENTS; i++) cmb_process_stop(i, 0);
         }
     }
-    CMB_FN bool demand(cmb::Sim &, uint32_t, uint32_t, int32_t) { return false; }
+    CMB_FN bool demand(S &, uint32_t, uint32_t, int32_t) { return false; }
 
-    CMB_FN void finish(cmb::Sim &sim, cmb::TrialOut &out)
+    CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         counter[6] = cmb_resourcepool_in_use(pool);
         for (uint32_t i = 0u; i < 8u; i++) out.counters[i] = counter[i];
@@ -134,6 +150,8 @@ struct PoolFight {
         out.max_queue = sim.fel_high;
     }
 };
+
+using PoolFight = PoolFightT<cmb::Sim>;
 
 // A template over the engine: QueueAndTideT<cmb::Sim> is the general-engine model (QueueAndTide); on the static tier it runs in the
 // second form with 8 processes and 2 spare event slots (the end event and the nuisance's interrupt), its priority queue in the

@@ -162,7 +162,10 @@ const char *cimba_b200_model_name(int model_id);
  * _GUARDED_RECORDED, _PRIOQ_RECORDED and _PRIOQ with the tier's priority queue and condition (the same workspace as their default
  * route at every capacity; a queue beyond the tier's tables is re-run on the general engine), and CIMBA_B200_MODEL_TIMERS with the
  * tier's timers, resume / yield, waits on processes and events and observers (same workspace as its default route; a trial that
- * needs a ninth spare event slot, or cancels a waited-on event in an order the tier does not keep, is re-run on the general engine) */
+ * needs a ninth spare event slot, or cancels a waited-on event in an order the tier does not keep, is re-run on the general engine),
+ * and CIMBA_B200_MODEL_PREEMPT, _BUFFER and _BUFFER_RECORDED on the tier's form with priorities, interrupts and pre-emption, the
+ * buffer's waiters in literal heaps (same workspace as their default route; a trial that needs a fifth spare event slot for model 4,
+ * a third for models 5 and 12, is re-run on the general engine) */
 #define CIMBA_B200_VARIANT_STATIC 17
 
 /* Error codes */

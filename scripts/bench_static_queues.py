@@ -1,9 +1,10 @@
-"""Events per second of the reference's queue programs on three routes of the library: the default fixed-capacity kernel with its
-repair pass (variant 0), the static tier (CIMBA_B200_VARIANT_STATIC) and the general engine (CIMBA_B200_VARIANT_GENERAL):
-test/test_objectqueue.c (models 3 and 11), test/test_priorityqueue.c (model 13) and the priority-queue-and-condition world of
-model 6.
+"""Events per second of the reference's queue and coverage programs on three routes of the library: the default fixed-capacity
+kernel with its repair pass (variant 0), the static tier (CIMBA_B200_VARIANT_STATIC) and the general engine
+(CIMBA_B200_VARIANT_GENERAL): test/test_objectqueue.c (models 3 and 11), test/test_priorityqueue.c (model 13), the
+priority-queue-and-condition world of model 6, test/test_resourcepool.c's cast with checks (model 4, preempt_kernel by default)
+and the buffer-and-resource world with test/test_buffer.c (models 5 and 12, buffer_kernel by default).
 
-    python scripts/bench_static_queues.py [--models 3,11,13,6] [--trials 506880] [--general-trials N]
+    python scripts/bench_static_queues.py [--models 3,11,13,6,4,5,12] [--trials 506880] [--general-trials N]
                                           [--engines default,static,general] [--reps 3] [--warmup 64] [--out F]
 
 * the card's name, power limit and SM clock, read with one nvidia-smi call before the runs;
@@ -12,12 +13,15 @@ model 6.
   the library call alone; the median events/s of each route and the ratios.  Each launch's time goes to stderr as it ends;
 * the last timed launch of each route compared row for row over the trials all ran (events, objects, clock, sums, counters), a
   SHA-256 of those rows, and diag[2] of the static route (trials its repair pass re-ran: 0 when the tier answered them all).
+  The run fails if the rows differ, or if the repair pass re-ran trials of a model the tier should answer alone at its shape -
+  every model but 4, whose route keeps four spare event slots (the fewest its vector cases need) and leaves the trials that
+  need a fifth, about 1.9 % at this shape, to the repair pass.
 
 Sizes (H100, 132 SMs): all three routes launch 64-lane CTAs.  The general engine runs at most CMB_RESIDENT_CTAS = 4 of them per
 SM - 33 792 lanes - and takes further trials grid-stride; the fixed-capacity kernel and the static tier launch one lane per trial,
 as many CTAs per SM as their registers allow.  The default 506 880 = 132 x 64 x 60 trials is a whole number of waves for any
 count of CTAs per SM that divides 60 (1-6, 10, 12, 15, 20), and a multiple of 33 792.  Capacity 10 and 500 time units per trial:
-about 4 200 events per trial.  Prints one JSON line; --out writes it to a file as well."""
+about 4 200 events per trial for the queue programs, 2 300 for model 4 and 4 500 / 5 800 for models 5 / 12.  Prints one JSON line; --out writes it to a file as well."""
 import argparse
 import hashlib
 import json
@@ -37,7 +41,11 @@ MASTER = 0x34F05C64D7AD598F
 SHAPE = {3: ("object queue test (test/test_objectqueue.c, no history)", 10, 500),
          11: ("object queue test (test/test_objectqueue.c)", 10, 500),
          13: ("priority queue test (test/test_priorityqueue.c)", 10, 500),
-         6: ("priority queue + condition (model 6)", 10, 500)}
+         6: ("priority queue + condition (model 6)", 10, 500),
+         4: ("pool with priorities, pre-emption and interrupts (test/test_resourcepool.c's cast, model 4)", 10, 500),
+         5: ("buffer + resource world (model 5)", 10, 500),
+         12: ("buffer test (test/test_buffer.c)", 10, 500)}
+REPAIRED_AT_SHAPE = {4}            # models whose static route leaves some trials of SHAPE to its repair pass (see above)
 VARIANT = {"default": 0, "static": cb.VARIANT_STATIC, "general": cb.VARIANT_GENERAL}
 
 
@@ -133,7 +141,7 @@ def main():
         Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         Path(a.out).write_text(line + "\n")
     for r in out["results"]:
-        assert r["bit_identical"] and r.get("static_repaired", 0) == 0, r["model"]
+        assert r["bit_identical"] and (r.get("static_repaired", 0) == 0 or r["model"] in REPAIRED_AT_SHAPE), r["model"]
 
 
 if __name__ == "__main__":
