@@ -62,7 +62,10 @@ namespace cmb {
 
 constexpr uint32_t NIL = 0xffffffffu;
 
-enum : uint32_t { TRIAL_ERR_ARENA = 64u };             // the HBM arena ran out: a container could not grow
+enum : uint32_t {
+    TRIAL_ERR_ARENA = 64u,              // the HBM arena ran out: a container could not grow
+    TRIAL_ERR_ARGUMENT = 128u,          // model code passed an argument the reference asserts against (an empty loaded die, an alias
+};                                      // table of 0 or more than its capacity entries)
 
 // ------------------------------------------------------------------------------------------------ arena
 // Growth memory shared by all trials of a launch: a bump allocator over a slice of the job's workspace.  Blocks a
@@ -1633,6 +1636,15 @@ CMB_FN double draw_erlang(S &sim, unsigned k, double mean)
 // slow paths per kernel); the static tier (cmb_static.cuh) overloads them inline, where a call would force its state into memory
 CMB_FN double draw_exponential(Sim &sim, double mean) { return gp_exponential(sim.rng, *sim.hot, mean); }
 CMB_FN double draw_std_normal(Sim &sim) { return gp_std_normal(sim.rng, *sim.hot); }
+
+// the face count of cmb_random_loaded_dice / _hyperexponential in model code: the reference asserts n > 0; here n = 0 flags the
+// trial (and the draw reads no array)
+template <class S>
+CMB_FN unsigned dice_faces(S &sim, unsigned n)
+{
+    if (n == 0u) sim.status |= TRIAL_ERR_ARGUMENT;
+    return n;
+}
 }  // namespace cmb
 }  // namespace cimba_b200
 
@@ -1756,14 +1768,38 @@ CMB_FN double draw_std_normal(Sim &sim) { return gp_std_normal(sim.rng, *sim.hot
 #define cmb_random_erlang(k, mean)          (cimba_b200::cmb::draw_erlang(sim, (k), (mean)))
 #define cmb_random_bernoulli(p)             (sim.rng.bernoulli(p))
 #define cmb_random_dice(lo, hi)             (sim.rng.dice((lo), (hi)))
-#define cmb_random_triangular(a, b, c)      (cimba_b200::rnd_triangular(sim.rng, (a), (b), (c)))
-#define cmb_random_rayleigh(s)              (cimba_b200::rnd_rayleigh(sim.rng, *sim.hot, (s)))
-#define cmb_random_PERT(lo, mode, hi)       (cimba_b200::rnd_PERT_mod(sim.rng, *sim.hot, (lo), (mode), (hi), 4.0))
-#define cmb_random_gamma(shape, scale)      (cimba_b200::rnd_gamma(sim.rng, *sim.hot, (shape), (scale)))
-#define cmb_random_beta(a, b, lo, hi)       (cimba_b200::rnd_beta(sim.rng, *sim.hot, (a), (b), (lo), (hi)))
-#define cmb_random_weibull(shape, scale)    (cimba_b200::rnd_weibull(sim.rng, *sim.hot, (shape), (scale)))
-#define cmb_random_lognormal(m, sd)         (cimba_b200::rnd_lognormal(sim.rng, *sim.hot, (m), (sd)))
-#define cmb_random_poisson(rate)            (cimba_b200::rnd_poisson(sim.rng, *sim.hot, (rate)))
+// the rest of cmb_random (include/cmb_random.h:189-940): one formulation over the sim's draws (distributions.cuh), out of line
+// on cmb::Sim, inline on the static tier; array arguments (ma, pa) are the model's own arrays
+#define cmb_random_std_exponential()        (cimba_b200::random_std_exponential(sim))
+#define cmb_random_triangular(a, b, c)      (cimba_b200::random_triangular(sim, (a), (b), (c)))
+#define cmb_random_rayleigh(s)              (cimba_b200::random_rayleigh(sim, (s)))
+#define cmb_random_PERT(lo, mode, hi)       (cimba_b200::random_PERT_mod(sim, (lo), (mode), (hi), 4.0))
+#define cmb_random_PERT_mod(lo, mode, hi, lambda) (cimba_b200::random_PERT_mod(sim, (lo), (mode), (hi), (lambda)))
+#define cmb_random_gamma(shape, scale)      (cimba_b200::random_gamma(sim, (shape), (scale)))
+#define cmb_random_std_gamma(shape)         (cimba_b200::random_std_gamma(sim, (shape)))
+#define cmb_random_beta(a, b, lo, hi)       (cimba_b200::random_beta(sim, (a), (b), (lo), (hi)))
+#define cmb_random_std_beta(a, b)           (cimba_b200::random_std_beta(sim, (a), (b)))
+#define cmb_random_weibull(shape, scale)    (cimba_b200::random_weibull(sim, (shape), (scale)))
+#define cmb_random_lognormal(m, sd)         (cimba_b200::random_lognormal(sim, (m), (sd)))
+#define cmb_random_logistic(m, s)           (cimba_b200::random_logistic(sim, (m), (s)))
+#define cmb_random_cauchy(mode, scale)      (cimba_b200::random_cauchy(sim, (mode), (scale)))
+#define cmb_random_hypoexponential(n, ma)   (cimba_b200::random_hypoexponential(sim, (n), (ma)))
+#define cmb_random_hyperexponential(n, ma, pa) (cimba_b200::random_hyperexponential(sim, cimba_b200::cmb::dice_faces(sim, (n)), (ma), (pa)))
+#define cmb_random_chisquared(k)            (cimba_b200::random_chisquared(sim, (k)))
+#define cmb_random_F_dist(a, b)             (cimba_b200::random_F_dist(sim, (a), (b)))
+#define cmb_random_std_t_dist(v)            (cimba_b200::random_std_t_dist(sim, (v)))
+#define cmb_random_t_dist(m, s, v)          (cimba_b200::random_t_dist(sim, (m), (s), (v)))
+#define cmb_random_pareto(shape, mode)      (cimba_b200::random_pareto(sim, (shape), (mode)))
+#define cmb_random_poisson(rate)            (cimba_b200::random_poisson(sim, (rate)))
+#define cmb_random_geometric(p)             (cimba_b200::random_geometric(sim, (p)))
+#define cmb_random_binomial(n, p)           (cimba_b200::random_binomial(sim, (n), (p)))
+#define cmb_random_negative_binomial(m, p)  (cimba_b200::random_negative_binomial(sim, (m), (p)))
+#define cmb_random_pascal(m, p)             (cimba_b200::random_negative_binomial(sim, (m), (p)))
+#define cmb_random_loaded_dice(n, pa)       (cimba_b200::random_loaded_dice(sim, cimba_b200::cmb::dice_faces(sim, (n)), (pa)))
+// struct cmb_random_alias as a model member of at most N entries: `cmb_random_alias<N> a;`, then cmb_random_alias_create(a, n, pa)
+// (Vose's tables built in place, the bits of cimba_b200_alias_create) and cmb_random_alias_sample(a)
+#define cmb_random_alias_create(a, n, pa)   ((void)((a).create((n), (pa)) || (sim.status |= cimba_b200::cmb::TRIAL_ERR_ARGUMENT)))
+#define cmb_random_alias_sample(a)          (cimba_b200::random_alias_sample(sim, (a).n, (a).uprob, (a).alias))
 #define cmb_resourcepool_available(rp)      ((rp).capacity - (rp).in_use)
 #define cmb_process_create(kind, prio, ctx) (sim.process_create((kind), (prio), (ctx)))
 #define cmb_process_start(pid)              (sim.process_start(pid))
@@ -1811,3 +1847,34 @@ CMB_FN double draw_std_normal(Sim &sim) { return gp_std_normal(sim.rng, *sim.hot
 #define cmb_condition_initialize(c)         (cimba_b200::cmb::condition_initialize(sim, (c)))
 #define cmb_condition_signal(c)             (cimba_b200::cmb::condition_signal(sim, m, (c)))
 #define cmb_resourceguard_register(g, obs)  (cimba_b200::cmb::guard_register(sim, m, (g), (obs)))
+
+// cmb_datasummary / cmb_wtdsummary (include/cmb_datasummary.h, include/cmb_wtdsummary.h) on summary.cuh's arithmetic: a model
+// member `cmb_datasummary s;`, the reference's calls through a pointer.  cmb_summary_to_counters(out, &s) writes either kind to
+// out.counters[0..7] as the row cimba_b200_merge_weighted_rows reads (a data summary's row has wsum = count).
+using cmb_datasummary = cimba_b200::SummaryAcc;
+using cmb_wtdsummary = cimba_b200::WtdAcc;
+template <unsigned N>
+using cmb_random_alias = cimba_b200::AliasTable<N>;
+#define cmb_datasummary_initialize(dsp)     ((void)(*(dsp) = cimba_b200::summary_empty()))
+#define cmb_datasummary_add(dsp, y)         (cimba_b200::summary_add_ptr((dsp), (y)))
+#define cmb_datasummary_merge(tgt, a, b)    (cimba_b200::summary_merge_ptr((tgt), (a), (b)))
+#define cmb_datasummary_count(dsp)          ((dsp)->count)
+#define cmb_datasummary_min(dsp)            ((dsp)->min)
+#define cmb_datasummary_max(dsp)            ((dsp)->max)
+#define cmb_datasummary_mean(dsp)           ((dsp)->m1)
+#define cmb_datasummary_variance(dsp)       (cimba_b200::summary_variance(*(dsp)))
+#define cmb_datasummary_stddev(dsp)         (cimba_b200::summary_stddev(*(dsp)))
+#define cmb_datasummary_skewness(dsp)       (cimba_b200::summary_skewness(*(dsp)))
+#define cmb_datasummary_kurtosis(dsp)       (cimba_b200::summary_kurtosis(*(dsp)))
+#define cmb_wtdsummary_initialize(wsp)      ((void)(*(wsp) = cimba_b200::wtd_empty()))
+#define cmb_wtdsummary_add(wsp, x, w)       (cimba_b200::wtd_add_ptr((wsp), (x), (w)))
+#define cmb_wtdsummary_merge(tgt, a, b)     (cimba_b200::wtd_merge_ptr((tgt), (a), (b)))
+#define cmb_wtdsummary_count(wsp)           ((wsp)->count)
+#define cmb_wtdsummary_min(wsp)             ((wsp)->min)
+#define cmb_wtdsummary_max(wsp)             ((wsp)->max)
+#define cmb_wtdsummary_mean(wsp)            ((wsp)->m1)
+#define cmb_wtdsummary_variance(wsp)        (cimba_b200::summary_variance(*(wsp)))
+#define cmb_wtdsummary_stddev(wsp)          (cimba_b200::summary_stddev(*(wsp)))
+#define cmb_wtdsummary_skewness(wsp)        (cimba_b200::summary_skewness(*(wsp)))
+#define cmb_wtdsummary_kurtosis(wsp)        (cimba_b200::summary_kurtosis(*(wsp)))
+#define cmb_summary_to_counters(out, sp)    (cimba_b200::summary_store_row(*(sp), (out).counters))

@@ -14,6 +14,9 @@
 //   * blocking calls are commands carried out by the dispatcher where the warp is together, and the ziggurat's slow path
 //     is taken by parked lanes in batches - as in the fused kernels (queue_model.cuh, whose shape this generalises); a hold
 //     of any distribution can be drawn there too (CMB_PROCESS_HOLD_SAMPLED: rectangles first, rewind + park + batch otherwise).
+//   * every cmb_random_* distribution, cmb_random_alias_* and cmb_datasummary_* / cmb_wtdsummary_* (cmb_device.cuh, bottom) inline
+//     here (inline_draws below): no call takes the generator's address, and in a sampler each of them - rejection loops included -
+//     gives up when a ziggurat draw leaves the rectangles (distributions.cuh), so CMB_PROCESS_HOLD_SAMPLED takes any of them.
 // A model that says `static constexpr bool static_interrupts = true;` gets the tier's second form (StaticSim<..., PRE = true>):
 // process priorities (cmb_process_create with a priority, cmb_process_priority_set), cmb_process_interrupt, CMB_RESOURCEPOOL_PREEMPT
 // and CMB_RESOURCE_PREEMPT, and - with a `static_holdables` hook naming its pools and resources - a process stopped or exiting
@@ -45,7 +48,7 @@
 // (test/test_resourcepool.c), coverage_models.cuh's PoolFightT (test/test_resourcepool.c's cast with checks) and
 // tutorial2_model.cuh (tutorial/tut_2_1.c), and with priority queues and conditions guarded_model.cuh (test/test_objectqueue.c,
 // test/test_priorityqueue.c) and coverage_models.cuh's QueueAndTideT; with static_waits coverage_models.cuh's FrontDeskT;
-// examples/tandem_model.cuh.
+// examples/tandem_model.cuh; examples/clinic_model.cuh (every cmb_random distribution, alias tables, summaries).
 #pragma once
 
 #include <type_traits>
@@ -390,6 +393,7 @@ struct StaticSim : StaticPriorities<NPROC, PRE>, StaticWaits<NPROC, W> {
     static constexpr int SLOTS = NPROC + NEVENT;
     static constexpr bool INTERRUPTS = PRE;
     static constexpr bool WAITS = W;
+    static constexpr bool inline_draws = true;      // every cmb_random_* inlines and honours hot_only (distributions.cuh)
     static_assert(NPROC >= 1 && NPROC <= 32, "a guard's wait list is a 32-bit mask of processes");
     static_assert(!PRE || NEVENT > 0, "interrupts and pre-emptions take spare event slots, and the event list must order by priority");
     static_assert(!W || PRE, "timers, resumes and waits on processes and events need the tier's second form (static_interrupts)");

@@ -14,7 +14,9 @@
 #pragma once
 
 #include <cfloat>
+#include <cmath>
 #include <cstdint>
+#include <cstring>
 #ifndef CMB_HOST_BUILD     // tests/cmb_engine_host.cpp compiles this text for the CPU
 #include <cuda_runtime.h>
 #endif
@@ -177,6 +179,101 @@ __host__ __device__ inline WtdAcc wtd_merge(const WtdAcc &a, const WtdAcc &b)
     return c;
 }
 
+// cmb_datasummary_add / _merge and cmb_wtdsummary_add / _merge as the reference calls them: through pointers, returning the count
+__host__ __device__ inline uint64_t summary_add_ptr(SummaryAcc *s, double y)
+{
+    summary_add(*s, y);
+    return s->count;
+}
+
+__host__ __device__ inline uint64_t summary_merge_ptr(SummaryAcc *tgt, const SummaryAcc *a, const SummaryAcc *b)
+{
+    *tgt = summary_merge(*a, *b);
+    return tgt->count;
+}
+
+__host__ __device__ inline uint64_t wtd_add_ptr(WtdAcc *s, double x, double w)
+{
+    wtd_add(*s, x, w);
+    return s->count;
+}
+
+__host__ __device__ inline uint64_t wtd_merge_ptr(WtdAcc *tgt, const WtdAcc *a, const WtdAcc *b)
+{
+    *tgt = wtd_merge(*a, *b);
+    return tgt->count;
+}
+
+// ---- the reference's statistics of a summary (include/cmb_datasummary.h, src/cmb_datasummary.c:214-249); cmb_wtdsummary's
+// delegate to the same moments (include/cmb_wtdsummary.h:192-197).  A is SummaryAcc, WtdAcc or the C ABI's
+// cimba_b200_datasummary: the host's cimba_b200_datasummary_* (capi.cu) and model code (cmb_datasummary_* in cmb_device.cuh)
+// both use these.
+template <class A>
+__host__ __device__ inline double summary_variance(const A &s)      // include/cmb_datasummary.h:197-210 (sample variance)
+{
+    return (s.count > 1u) ? s.m2 / (double)(s.count - 1u) : 0.0;
+}
+
+template <class A>
+__host__ __device__ inline double summary_stddev(const A &s)
+{
+    return sqrt(summary_variance(s));
+}
+
+template <class A>
+__host__ __device__ inline double summary_skewness(const A &s)      // :214-230: population estimate, then the finite-sample correction
+{
+    if (s.count <= 2u) return 0.0;
+    const double n = (double)s.count;
+    const double g = sqrt(n) * s.m3 / pow(s.m2, 1.5);
+    return sqrt(n * (n - 1.0)) * g / (n - 2.0);
+}
+
+template <class A>
+__host__ __device__ inline double summary_kurtosis(const A &s)      // :233-249: sample excess kurtosis
+{
+    if (s.count <= 3u) return 0.0;
+    const double n = (double)s.count;
+    const double g = n * s.m4 / (s.m2 * s.m2) - 3.0;
+    return (n - 1.0) / ((n - 2.0) * (n - 3.0)) * ((n + 1.0) * g + 6.0);
+}
+
+// A summary as one trial's 8-word row of counters: {count (u64), min, max, m1, m2, m3, m4, wsum (f64 bit patterns)} - what
+// cimba_b200_merge_weighted_rows reads.  A cmb_datasummary's row carries wsum = count: the weighted merge with weights equal to
+// the counts is the unweighted merge (src/cmb_wtdsummary.c:152-194 with w = n is src/cmb_datasummary.c:93-131, term for term).
+__host__ __device__ inline uint64_t summary_bits(double d)
+{
+#ifdef __CUDA_ARCH__
+    return (uint64_t)__double_as_longlong(d);
+#else
+    uint64_t u;
+    memcpy(&u, &d, sizeof u);
+    return u;
+#endif
+}
+
+__host__ __device__ inline void wtd_store_row(const WtdAcc &a, uint64_t *row)
+{
+    row[0] = a.count;
+    row[1] = summary_bits(a.min);
+    row[2] = summary_bits(a.max);
+    row[3] = summary_bits(a.m1);
+    row[4] = summary_bits(a.m2);
+    row[5] = summary_bits(a.m3);
+    row[6] = summary_bits(a.m4);
+    row[7] = summary_bits(a.wsum);
+}
+
+__host__ __device__ inline void summary_store_row(const WtdAcc &a, uint64_t *row)
+{
+    wtd_store_row(a, row);
+}
+
+__host__ __device__ inline void summary_store_row(const SummaryAcc &a, uint64_t *row)
+{
+    wtd_store_row(WtdAcc{a.count, a.min, a.max, a.m1, a.m2, a.m3, a.m4, (double)a.count}, row);
+}
+
 // A fused cmb_timeseries (src/cmb_timeseries.c:106-188): a new sample fixes the duration of
 // the previous one, and that (x, duration) pair is all cmb_timeseries_summarize feeds to
 // cmb_wtdsummary_add - so the history itself is never stored.
@@ -258,18 +355,6 @@ __device__ inline WtdAcc wtd_load_row(const uint64_t *row)
     a.m4 = __longlong_as_double((long long)row[6]);
     a.wsum = __longlong_as_double((long long)row[7]);
     return a;
-}
-
-__device__ inline void wtd_store_row(const WtdAcc &a, uint64_t *row)
-{
-    row[0] = a.count;
-    row[1] = (uint64_t)__double_as_longlong(a.min);
-    row[2] = (uint64_t)__double_as_longlong(a.max);
-    row[3] = (uint64_t)__double_as_longlong(a.m1);
-    row[4] = (uint64_t)__double_as_longlong(a.m2);
-    row[5] = (uint64_t)__double_as_longlong(a.m3);
-    row[6] = (uint64_t)__double_as_longlong(a.m4);
-    row[7] = (uint64_t)__double_as_longlong(a.wsum);
 }
 
 __device__ inline void wtd_block_reduce(WtdAcc acc, uint64_t *out_row)

@@ -113,15 +113,8 @@ struct CheeseT {
     CMB_FN void finish(S &sim, cmb::TrialOut &out)
     {
         cmb_resourcepool_stop_recording(cheese);
-        const WtdAcc &h = cheese.history.acc;           // what cmb_timeseries_summarize makes of the stored history
-        out.counters[0] = h.count;
-        out.counters[1] = (uint64_t)__double_as_longlong(h.min);
-        out.counters[2] = (uint64_t)__double_as_longlong(h.max);
-        out.counters[3] = (uint64_t)__double_as_longlong(h.m1);
-        out.counters[4] = (uint64_t)__double_as_longlong(h.m2);
-        out.counters[5] = (uint64_t)__double_as_longlong(h.m3);
-        out.counters[6] = (uint64_t)__double_as_longlong(h.m4);
-        out.counters[7] = (uint64_t)__double_as_longlong(h.wsum);
+        const cmb_wtdsummary &h = cheese.history.acc;   // what cmb_timeseries_summarize makes of the stored history
+        cmb_summary_to_counters(out, &h);
         out.objects = successes;
         out.sum_wait = sum_time;
         out.max_queue = (uint32_t)h.count;

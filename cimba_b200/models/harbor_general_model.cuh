@@ -22,7 +22,7 @@ struct HarborGeneral {
     cmb::Tag active_store[9];
     uint32_t departed;                                          // LIFO of departed ships (through Process::u[1]), NIL = empty
     uint32_t weather, tide, arrivals, departures, dots;
-    SummaryAcc through[2];                                      // trl->system_time[size]
+    cmb_datasummary through[2];                                      // trl->system_time[size]
     double   arr_mean, unload_small, sum_system_time;
     uint64_t cnt, alive, most_alive, reactivated, left[2];
     enum : uint32_t { WEATHER, TIDE, ARRIVALS, SHIP, DEPARTURES, DOTS };
@@ -138,7 +138,7 @@ struct HarborGeneral {
                 departed = (uint32_t)sim.proc[ship].u[1];
                 const double t_sys = sim.proc[ship].f[1];       // cmb_process_exit_value
                 const uint32_t size = sim.proc[ship].ctx;
-                summary_add(through[size], t_sys);
+                (void)cmb_datasummary_add(&through[size], t_sys);
                 sum_system_time += t_sys;
                 left[size] += 1u;
                 cmb_process_destroy(ship);
@@ -167,8 +167,8 @@ struct HarborGeneral {
         sum_system_time = 0.0;
         cnt = alive = most_alive = reactivated = 0u;
         left[0] = left[1] = 0u;
-        through[0] = summary_empty();
-        through[1] = summary_empty();
+        cmb_datasummary_initialize(&through[0]);
+        cmb_datasummary_initialize(&through[1]);
         departed = cmb::NIL;
         weather = cmb_process_create(WEATHER, 0, 0u);
         cmb_process_start(weather);
@@ -230,8 +230,8 @@ struct HarborGeneral {
     {
         out.counters[0] = left[0];
         out.counters[1] = left[1];
-        out.counters[2] = (uint64_t)__double_as_longlong(through[0].m1);
-        out.counters[3] = (uint64_t)__double_as_longlong(through[1].m1);
+        out.counters[2] = (uint64_t)__double_as_longlong(cmb_datasummary_mean(&through[0]));
+        out.counters[3] = (uint64_t)__double_as_longlong(cmb_datasummary_mean(&through[1]));
         out.counters[4] = tugs.history.acc.count;       // history samples with a duration (recording is never stopped)
         out.counters[5] = (uint64_t)__double_as_longlong(tugs.history.acc.m1);
         out.counters[6] = berths[0].history.acc.count | (berths[1].history.acc.count << 32);

@@ -74,15 +74,7 @@ struct MM1RecordedT {
     {
         MM1RecordedT &m = *this;
         cmb_objectqueue_recording_stop(queue);
-        const WtdAcc &h = queue.history.acc;            // what cmb_timeseries_summarize makes of the stored history
-        out.counters[0] = h.count;
-        out.counters[1] = (uint64_t)__double_as_longlong(h.min);
-        out.counters[2] = (uint64_t)__double_as_longlong(h.max);
-        out.counters[3] = (uint64_t)__double_as_longlong(h.m1);
-        out.counters[4] = (uint64_t)__double_as_longlong(h.m2);
-        out.counters[5] = (uint64_t)__double_as_longlong(h.m3);
-        out.counters[6] = (uint64_t)__double_as_longlong(h.m4);
-        out.counters[7] = (uint64_t)__double_as_longlong(h.wsum);
+        cmb_summary_to_counters(out, &queue.history.acc);   // what cmb_timeseries_summarize makes of the stored history
         cmb_process_stop(service, 0);
         out.objects = obj_cnt;
         out.sum_wait = sum_wait;

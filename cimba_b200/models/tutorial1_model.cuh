@@ -92,15 +92,7 @@ struct Tutorial1T {
 
     CMB_FN void finish(S &, cmb::TrialOut &out)                          // :205-209: cmb_timeseries_summarize of the history
     {
-        const WtdAcc &h = que.history.acc;
-        out.counters[0] = h.count;
-        out.counters[1] = (uint64_t)__double_as_longlong(h.min);
-        out.counters[2] = (uint64_t)__double_as_longlong(h.max);
-        out.counters[3] = (uint64_t)__double_as_longlong(h.m1);                 // avg_queue_length
-        out.counters[4] = (uint64_t)__double_as_longlong(h.m2);
-        out.counters[5] = (uint64_t)__double_as_longlong(h.m3);
-        out.counters[6] = (uint64_t)__double_as_longlong(h.m4);
-        out.counters[7] = (uint64_t)__double_as_longlong(h.wsum);
+        cmb_summary_to_counters(out, &que.history.acc);                         // counters[3] = avg_queue_length
         out.objects = units_put;
         out.sum_wait = (double)units_got;
     }
