@@ -1858,6 +1858,21 @@ CMB_FN void static_finish_command(S &sim, Model &m, int who, uint32_t cmd)
     }
 }
 
+// cmb_random_flip's cache, where the sim keeps one (StaticSim<..., PRE = true>): the dispatcher saves it with the generator before
+// it tries a sampler with the rectangles only, and puts both back when the sampler gives up, so that the repeat sees the flips the
+// first try saw
+template <class S, class = void>
+struct FlipState {
+    CMB_FN explicit FlipState(const S &) {}
+    CMB_FN void restore(S &) const {}
+};
+template <class S>
+struct FlipState<S, decltype((void)std::declval<S &>().flips)> {
+    FlipCache saved;
+    CMB_FN explicit FlipState(const S &sim) : saved(sim.flips) {}
+    CMB_FN void restore(S &sim) const { sim.flips = saved; }
+};
+
 // `static constexpr bool static_interrupts = true;` in a model: its static-tier form is StaticSim<..., PRE = true>
 template <class Model, class = void>
 struct StaticInterrupts {
@@ -1913,6 +1928,7 @@ inline void static_run_trial_host(S &sim, Model &m, const TrialIn &in, TrialOut 
         else if (cmd == CMD_HOLD_SAMPLED) {
             // as the device does it: the rectangles only first, and if they do not suffice the generator rewound and the whole sampler again
             const Sfc64 saved = sim.rng;
+            const FlipState<S> saved_flips(sim);            // a sampler may call cmb_random_flip() before a draw gives up
             sim.hot_only = true;
             sim.hot_failed = false;
             double dur = ModelSampler<Model, S>::draw(m, sim, sim.cmd_sample);
@@ -1920,6 +1936,7 @@ inline void static_run_trial_host(S &sim, Model &m, const TrialIn &in, TrialOut 
             if (sim.hot_failed) {
                 sim.hot_failed = false;
                 sim.rng = saved;
+                saved_flips.restore(sim);
                 dur = ModelSampler<Model, S>::draw(m, sim, sim.cmd_sample);
             }
             if (dur < 0.0) sim.status |= TRIAL_ERR_NEGATIVE_HOLD;
@@ -2063,6 +2080,7 @@ static_trial_kernel(const StaticArgs sa)
         // draw needs more rewinds the generator and parks
         if (sampled) {
             const Sfc64 saved = sim.rng;
+            const FlipState<S> saved_flips(sim);            // a sampler may call cmb_random_flip() before a draw gives up
             sim.hot_only = true;
             sim.hot_failed = false;
             const double dur = ModelSampler<ModelT<S>, S>::draw(m, sim, sim.cmd_sample);
@@ -2070,6 +2088,7 @@ static_trial_kernel(const StaticArgs sa)
             if (sim.hot_failed) {
                 sim.hot_failed = false;
                 sim.rng = saved;
+                saved_flips.restore(sim);
                 parked = true;
                 parked_sampled = true;
                 parked_who = who;

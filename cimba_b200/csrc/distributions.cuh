@@ -178,6 +178,12 @@ __device__ __forceinline__ double random_hyperexponential(S &s, unsigned n, cons
     return n > 0u ? draw_exponential(s, ma[ui]) : 0.0;
 }
 
+// A CPU build of this text may define CMB_OBSERVE_SQUEEZE(lhs, rhs, d, log_w) to see each of the Marsaglia-Tsang loop's log
+// comparisons (tests/random_sweep_host.cpp measures how close they come to a tie); elsewhere it is nothing.
+#ifndef CMB_OBSERVE_SQUEEZE
+#define CMB_OBSERVE_SQUEEZE(lhs, rhs, d, log_w) ((void)0)
+#endif
+
 // Marsaglia & Tsang, src/cmb_random.c:465-497
 template <class S>
 __device__ __forceinline__ double std_gamma_loop(S &s, double shape)
@@ -193,8 +199,14 @@ __device__ __forceinline__ double std_gamma_loop(S &s, double shape)
         } while (v <= 0.0);
         const double w = v * v * v;
         const double u = draw_uniform01(s);
-        if ((u < 1.0 - 0.331 * (x * x) * (x * x))
-            || (log(u) < (0.5 * x * x) + (d * (1.0 - w + log(w))))) {
+        if (u < 1.0 - 0.331 * (x * x) * (x * x)) {
+            return d * w;
+        }
+        const double lhs = log(u);
+        const double log_w = log(w);
+        const double rhs = (0.5 * x * x) + (d * (1.0 - w + log_w));
+        CMB_OBSERVE_SQUEEZE(lhs, rhs, d, log_w);
+        if (lhs < rhs) {
             return d * w;
         }
     }
@@ -316,12 +328,15 @@ __device__ __forceinline__ double random_rayleigh(S &s, double sc)
     return sqrt(x * x + y * y);
 }
 
-// :558-573
+// :558-573.  The reference returns (unsigned)ceil(...), and for p below about 1e-9 the quotient passes 2^32 (nearly always at
+// p = 1e-12; p > 0 is all the reference asks).  That conversion is undefined in C (C11 6.3.1.4); the reference's build, gcc on
+// x86-64, wraps it modulo 2^32 where the device's cvt.rzi.u32.f64 would saturate at 4294967295: x86_cvttsd2si (rng.cuh) states
+// the wrap.
 template <class S>
 __device__ __forceinline__ unsigned random_geometric(S &s, double p)
 {
     const double denom = -log(1.0 - p);
-    return (unsigned)ceil(draw_exponential(s, 1.0) / denom);
+    return (unsigned)(uint64_t)x86_cvttsd2si(ceil(draw_exponential(s, 1.0) / denom));
 }
 
 // :576-588

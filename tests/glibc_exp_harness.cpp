@@ -23,8 +23,15 @@ int main(int argc, char **argv)
     const long n = argc > 1 ? std::atol(argv[1]) : 2000000;
     unsigned long bad = 0;
     for (long i = 0; i < n; i++) {
-        const double scale = (i & 3) == 0 ? 700.0 : ((i & 3) == 1 ? 40.0 : ((i & 3) == 2 ? 8.0 : 1.0e-3));
+        // the first quarter reaches past the overflow (709.78) and underflow (-745.13) thresholds: glibc's special case
+        const double scale = (i & 3) == 0 ? 760.0 : ((i & 3) == 1 ? 40.0 : ((i & 3) == 2 ? 8.0 : 1.0e-3));
         const double x = (double)(int64_t)next64() / 9.3e18 * scale;
+        const double a = std::exp(x), b = cimba_b200::glibc_exp(x);
+        if (std::memcmp(&a, &b, 8) != 0) bad++;
+    }
+    const double edges[] = {0.0, -0.0, 0x1p-55, -0x1p-55, 512.0, -512.0, 1024.0, -1024.0, 1e308, -1e308, 709.782712893384,
+                            709.7827128933841, -708.3964185322641, -745.1332191019411, -745.1332191019412, INFINITY, -INFINITY, NAN};
+    for (const double x : edges) {
         const double a = std::exp(x), b = cimba_b200::glibc_exp(x);
         if (std::memcmp(&a, &b, 8) != 0) bad++;
     }
