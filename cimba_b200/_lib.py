@@ -85,6 +85,7 @@ SYMBOLS = {
     "cimba_b200_workspace_bytes": (C.c_uint64, [C.POINTER(DeviceJob)]),
     "cimba_b200_launch": (C.c_int, [C.POINTER(DeviceJob), C.c_void_p]),
     "cimba_b200_launch_count": (C.c_uint64, []),
+    "cimba_b200_mm1_resident_ctas": (C.c_int, [C.c_int]),
     "cimba_b200_summarize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
     "cimba_b200_run_experiment": (C.c_int, [C.c_void_p, C.c_uint64, C.c_size_t, C.POINTER(Experiment)]),
     "cimba_b200_release_cache": (None, []),
@@ -132,6 +133,10 @@ SYMBOLS = {
 }
 
 
+# diagnostics that builds older than this binding lack (CIMBA_B200_LIB may select one to compare against): left unbound there
+DIAGNOSTICS = {"cimba_b200_mm1_resident_ctas"}
+
+
 def load() -> C.CDLL:
     if not LIB_PATH.exists():
         raise ImportError(
@@ -139,6 +144,8 @@ def load() -> C.CDLL:
             "(nvcc, sm_90a). cimba_b200 has no CPU fallback.")
     lib = C.CDLL(str(LIB_PATH))
     for name, (res, args) in SYMBOLS.items():
+        if name in DIAGNOSTICS and not hasattr(lib, name):
+            continue
         fn = getattr(lib, name)          # AttributeError if the export is missing
         fn.restype = res
         fn.argtypes = args

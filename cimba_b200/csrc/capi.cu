@@ -389,6 +389,22 @@ uint64_t queue_rings_bytes(const cimba_b200_device_job *job)
 
 uint64_t queue_workspace(const cimba_b200_device_job *job) { return cmb::rings_then_arena(queue_rings_bytes(job), repair_arena_bytes(job)); }
 
+// 8 CTAs of mm1_kernel per SM (65 536 trials in one wave on 132 SMs) need 8 x (27 136 + 1 024) B = 220 KB of shared memory,
+// which only the largest carveout gives; with a smaller split the driver might pick, the launch would take two waves.  Both
+// instantiations ask for it, once per device (about 28 KB of the SM's unified L1 / shared memory stay L1).
+int mm1_prefer_shared()
+{
+    static std::atomic<uint64_t> done{0};           // one bit per device
+    int dev = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    const uint64_t bit = dev < 64 ? 1ull << dev : 0ull;
+    if (bit != 0u && (done.load() & bit) != 0u) return CIMBA_B200_OK;
+    CUDA_TRY(cudaFuncSetAttribute(mm1_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    CUDA_TRY(cudaFuncSetAttribute(mm1_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    done.fetch_or(bit);
+    return CIMBA_B200_OK;
+}
+
 int queue_launch(const cimba_b200_device_job *job, cudaStream_t st)
 {
     if (const int e = check_workspace(job)) return e;
@@ -427,6 +443,7 @@ int queue_launch(const cimba_b200_device_job *job, cudaStream_t st)
         e = launch_kernel(job, mm1_pc_kernel<false>, mm1_pc_kernel<true>, pc_grid, 2 * MM1_PC_CONSUMERS, 0, st, qa, "mm1_kernel launch");
     }
     else {
+        if (const int c = mm1_prefer_shared()) return c;
         e = launch_kernel(job, mm1_kernel<false>, mm1_kernel<true>, grid, QUEUE_BLOCK, 0, st, qa, "mm1_kernel launch");
     }
     return then_repair<models::MM1>(e, job, rings, st, "repair pass (M/M/1)");
@@ -719,6 +736,15 @@ extern "C" {
 const char *cimba_b200_version(void) { return CIMBA_B200_VERSION_STRING; }
 const char *cimba_b200_last_error(void) { return g_err; }
 uint64_t cimba_b200_launch_count(void) { return g_launches.load(); }
+
+int cimba_b200_mm1_resident_ctas(int trace)
+{
+    if (const int e = mm1_prefer_shared()) return e;
+    int per_sm = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, trace ? mm1_kernel<true> : mm1_kernel<false>, QUEUE_BLOCK, 0));
+    return per_sm;
+}
+
 uint64_t cimba_b200_fmix64(uint64_t seed, uint64_t nonce) { return fmix64(seed, nonce); }
 
 int cimba_b200_device_count(void)

@@ -35,6 +35,15 @@ namespace cimba_b200 {
 #define MM1_STEPS 8            // event steps per loop iteration (a multiple or a divisor of MM1_PARK_MASK + 1)
 #endif
 
+// Shared-memory ring entries per trial.  A take that leaves more than this many waiting refills the freed slot from the
+// trial's HBM ring, a round trip the whole warp waits for; at rho = 0.9 a queue passes 48 about 1 / 0.9^16 = 5.4 times
+// less often than it passes 32.  The ring (one row of QUEUE_BLOCK doubles per entry), the row that takes the stores of
+// lanes that do not put, and the ziggurat table come to 27 136 B: 8 CTAs + the 1 KB the hardware reserves per CTA fit the
+// 228 KB an SM has when the kernel asks for the largest shared-memory carveout (capi.cu does).
+constexpr int MM1_WINDOW = 48;
+static_assert(8 * ((MM1_WINDOW + 1) * QUEUE_BLOCK * 8 + 256 * 8 + 1024) <= 228 * 1024,
+              "8 CTAs of mm1_kernel must fit an SM: 65 536 trials in one wave on 132 SMs");
+
 // 32-bit shared-window accesses: one address register, no generic->shared
 // conversion per access (the static-__shared__ form costs extra
 // instructions each time).
@@ -63,7 +72,7 @@ __global__ void __launch_bounds__(QUEUE_BLOCK)
 mm1_kernel(const QueueArgs a)
 {
     __shared__ double exp_x[256];                       // ziggurat layer widths (hot table)
-    __shared__ double ring_smem[QUEUE_WINDOW * QUEUE_BLOCK];
+    __shared__ double ring_smem[(MM1_WINDOW + 1) * QUEUE_BLOCK];   // MM1_WINDOW rows of ring, then the scratch row
 
     for (unsigned i = threadIdx.x; i < 256u; i += blockDim.x) {
         exp_x[i] = zig::zig_exp_x[i];
@@ -71,7 +80,6 @@ mm1_kernel(const QueueArgs a)
     __syncthreads();
 
     constexpr unsigned FULL = 0xffffffffu;
-    constexpr uint32_t WMASK = QUEUE_WINDOW - 1;
     constexpr uint32_t ROW = QUEUE_BLOCK * 8u;          // bytes between consecutive ring entries of one trial
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
     const unsigned lane = threadIdx.x & 31u;
@@ -103,11 +111,16 @@ mm1_kernel(const QueueArgs a)
     // at the moment an arrival puts (it otherwise always owns one pending event).
     uint32_t produced = 0u, served = 0u, dropped = 0u, status = TRIAL_OK, longest = 0u;
     const uint32_t quota = (uint32_t)a.num_objects;
-    uint32_t win = (uint32_t)__cvta_generic_to_shared(&ring_smem[threadIdx.x]);
+    // The window's tail and head slots (`produced` and `served` modulo MM1_WINDOW) as byte offsets from the ring's start,
+    // the lane's column included, advanced wherever the counters are.  Every offset stays in the ring, a void trial's too.
+    const uint32_t ring = (uint32_t)__cvta_generic_to_shared(&ring_smem[0]);
+    uint32_t tail = threadIdx.x * 8u, head = threadIdx.x * 8u;
+    const uint32_t scratch = MM1_WINDOW * ROW + threadIdx.x * 8u;   // sink for the store of lanes that do not put
+    // the next slot: off + ROW, or back to the first row from the last, where off + ROW - MM1_WINDOW * ROW is the smaller
+    // (below the last row it wraps past 2^32)
+    const auto next_slot = [](uint32_t off) { return min(off + ROW, off - (MM1_WINDOW - 1) * ROW); };
     uint32_t tab = (uint32_t)__cvta_generic_to_shared(&exp_x[0]);
-    __shared__ double scratch_smem[QUEUE_BLOCK];        // sink for the store of lanes that do not put
-    uint32_t scratch = (uint32_t)__cvta_generic_to_shared(&scratch_smem[threadIdx.x]);
-    asm volatile("" : "+r"(win), "+r"(tab), "+r"(scratch));     // keep in registers (no per-step rematerialisation)
+    asm volatile("" : "+r"(tab));                       // keep in a register (no per-step rematerialisation)
     double *const spill = (a.spill_cap && alive) ? a.spill + trial * a.spill_cap : nullptr;
     const uint32_t spill_mask = a.spill_cap - 1u;
 
@@ -168,9 +181,12 @@ mm1_kernel(const QueueArgs a)
         const uint32_t p0 = produced, s0 = served;
         const uint32_t q_len = p0 - s0;
         const bool put = is_arr & wake;
-        const bool put_far = put & (q_len >= (uint32_t)QUEUE_WINDOW);
-        sts_f64((put & !put_far) ? win + (p0 & WMASK) * ROW : scratch, now);
-        if (put) produced++;
+        const bool put_far = put & (q_len >= (uint32_t)MM1_WINDOW);
+        sts_f64(ring + ((put & !put_far) ? tail : scratch), now);
+        if (put) {
+            produced++;
+            tail = next_slot(tail);
+        }
         // cmb_objectqueue_put -> cmb_resourceguard_signal(front guard): wake the server
         if (put & (k_srv == 0u)) {
             issued++;
@@ -183,13 +199,14 @@ mm1_kernel(const QueueArgs a)
         if (is_srv & wake) sum_wait = new_sum;          // back from the service hold
         // cmb_objectqueue_get: take the head, or wait at the front guard (slot stays empty)
         const bool take = is_srv & (q_len != 0u);
-        const uint32_t head_slot = win + (s0 & WMASK) * ROW;
-        const double head_stamp = lds_f64(head_slot);   // harmless when the ring is empty
+        const uint32_t h0 = head;
+        const double head_stamp = lds_f64(ring + h0);   // harmless when the ring is empty
         if (take) {
             stamp = head_stamp;
             served++;
+            head = next_slot(head);
         }
-        const bool refill_far = take & (q_len > (uint32_t)QUEUE_WINDOW);
+        const bool refill_far = take & (q_len > (uint32_t)MM1_WINDOW);
 
         // ---------------- hold: consume the look-ahead variate, insert the wake-up
         const bool draw = take | (is_arr & (produced < quota));
@@ -207,15 +224,16 @@ mm1_kernel(const QueueArgs a)
         // ---------------- rare: the queue reaches past the on-chip window
         if (put_far | refill_far) {
             if (refill_far) {                           // refill the freed slot from HBM
-                sts_f64(head_slot, spill[(s0 + QUEUE_WINDOW) & spill_mask]);
+                sts_f64(ring + h0, spill[(s0 + MM1_WINDOW) & spill_mask]);
             }
-            else if (spill != nullptr && q_len - QUEUE_WINDOW <= spill_mask) {
+            else if (spill != nullptr && q_len - MM1_WINDOW <= spill_mask) {
                 spill[p0 & spill_mask] = now;
             }
             else {
                 status |= TRIAL_ERR_QUEUE_OVERFLOW;     // entry dropped: the trial is void from here on
                 dropped++;
                 served++;                               // keep produced - served = entries actually stored
+                head = next_slot(head);
             }
         }
         longest = max(longest, produced - served);

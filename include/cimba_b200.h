@@ -283,6 +283,11 @@ int cimba_b200_launch(const cimba_b200_device_job *job, void *stream);
 /* Number of kernels this library has launched so far in this process. */
 uint64_t cimba_b200_launch_count(void);
 
+/* CTAs of the M/M/1 trial kernel (MODEL_MM1, variant 0; trace != 0: its pop-recording form) resident per SM of the
+ * current device, with the shared-memory carveout the library asks for before it launches them: a diagnostic.
+ * Negative: an error code. */
+int cimba_b200_mm1_resident_ctas(int trace);
+
 /* Reduce per-trial results to a cmb_datasummary of avg = sum_wait/objects on
  * the device (benchmark/MM1_multi.c:143-148 does this with a serial host loop).
  * out_summary: DEVICE pointer to 8 doubles {count, min, max, m1, m2, m3, m4, 0}.
