@@ -11,11 +11,12 @@
 // merging those regions' results.  With few warps per scheduler the kernel is
 // bound by dependent-issue latency.  Here one event step is a single
 // straight-line, predicated sequence that all 32 lanes execute together:
-//   pop-min over the two process-owned event slots (compare + selects),
-//   the arrival body and the service body as predicated updates of the same
-//   registers (a lane is in exactly one of them), the variate draw and the
-//   wake-up insert.  The only branches left are the rare ones: queue spill to
-//   HBM, trial completion and the parked ziggurat slow path.
+//   the pop of the first of the two pending events, which are kept in time
+//   order, the arrival body and the service body as predicated updates of the
+//   same registers (a lane is in exactly one of them), the variate draw and the
+//   wake-up insert (one compare and selects).  The only branches left are the
+//   look-ahead refill and the rare ones: queue spill to HBM, trial completion
+//   and the parked ziggurat slow path.
 #pragma once
 
 #include "engine.cuh"
@@ -62,6 +63,7 @@ __device__ __forceinline__ double lds_f64(uint32_t addr)
 // Event keys carry the action in their two low bits: key = (issue counter << 2) | action.
 // Counters are unique, so ordering by this word is ordering by issue counter (the
 // reference's FIFO tie-break, src/cmi_hashheap.c:55-80) and one register holds both.
+// A key issued later is the larger, as long as the counter stays below 2^30.
 __device__ __forceinline__ uint32_t pack_key(uint32_t counter, uint32_t action)
 {
     return (counter << 2) | action;
@@ -98,16 +100,23 @@ mm1_kernel(const QueueArgs a)
     // ---- per-trial state (registers)
     Sfc64 rng;
     rng.a = rng.b = rng.c = rng.d = 0u;
-    // event slot 0 = arrival process, slot 1 = service process; an empty slot has
-    // time +inf and key 0 (action ACT_NONE)
-    double t_arr = INF, t_srv = INF;
-    uint32_t k_arr = 0u, k_srv = 0u;
-    uint32_t issued = 0u;                               // item_counter, src/cmi_hashheap.c:449-453
+    // The two pending events in pop order: slot 0 is the next to pop, slot 1 the other.  Each process owns at most one
+    // pending event, so the two slots belong to different processes, and one word says which: slot 0 is the arrival
+    // process's when `lead_arr` is 1, the service process's when it is 0.  An empty slot has time +inf and key 0 (action
+    // ACT_NONE) and belongs to the process that has no event pending.
+    double t0 = INF, t1 = INF;
+    uint32_t k0 = 0u, k1 = 0u;
+    uint32_t lead_arr = 1u;
+    // item_counter (src/cmi_hashheap.c:449-453) kept as the WAKE_TIME key of the last counter issued,
+    // (counter << 2) | ACT_WAKE_TIME, so that issuing a key is one add of 4.  The word wraps when the counter reaches
+    // 2^30, as the keys do; `wraps` counts that (once per loop iteration, which issues far fewer than 2^30 keys), so the
+    // event count written after the loop is exact.
+    uint32_t last_key = ACT_WAKE_TIME, last_seen = ACT_WAKE_TIME, wraps = 0u;
     double now = 0.0, stamp = 0.0, sum_wait = 0.0;
     double arr_mean = 1.0, srv_mean = 1.0;
     // FIFO discipline: the k-th object put is the k-th object taken, so the ring's
     // tail index is `produced`, its head index is `served`, its length their difference.
-    // The server is waiting at the front guard exactly when its event slot is empty
+    // The server is waiting at the front guard exactly when no other event is pending
     // at the moment an arrival puts (it otherwise always owns one pending event).
     uint32_t produced = 0u, served = 0u, dropped = 0u, status = TRIAL_OK, longest = 0u;
     const uint32_t quota = (uint32_t)a.num_objects;
@@ -143,9 +152,9 @@ mm1_kernel(const QueueArgs a)
         arr_mean = a.arr_mean[trial];
         srv_mean = a.srv_mean[trial];
         rng.seed(fmix64(a.master_seed, a.first_trial + trial));
-        t_arr = 0.0; k_arr = pack_key(1u, ACT_START);   // cmb_process_start(arrival), MM1_multi.c:107-108
-        t_srv = 0.0; k_srv = pack_key(2u, ACT_START);   // cmb_process_start(service), :109-111
-        issued = 2u;
+        t0 = 0.0; k0 = pack_key(1u, ACT_START);         // cmb_process_start(arrival), MM1_multi.c:107-108
+        t1 = 0.0; k1 = pack_key(2u, ACT_START);         // cmb_process_start(service), :109-111
+        last_key = last_seen = pack_key(2u, ACT_WAKE_TIME);
         refill();
     }
 
@@ -157,23 +166,22 @@ mm1_kernel(const QueueArgs a)
     // One event step.  A lane that is finished or parked runs it with every update predicated off, so the registers of a
     // finished trial hold its results until they are written after the loop.
     const auto event_step = [&]() {
-        // ---------------- pop-min (cmi_hashheap_dequeue order: time asc, key asc)
+        // ---------------- pop (cmi_hashheap_dequeue order: time asc, key asc): slot 0
         const bool go0 = flags == 1u;                   // alive and not parked
-        const bool first_arr = (t_arr < t_srv) | ((t_arr == t_srv) & (k_arr < k_srv));
-        const uint32_t key = first_arr ? k_arr : k_srv;
+        const uint32_t key = k0;
         const bool go = go0 & (key != 0u);
         if (go0 & (key == 0u)) flags = 0u;              // event list ran dry: the trial is over
-        const bool is_arr = go & first_arr;
-        const bool is_srv = go & !first_arr;
+        const bool is_arr = go & (lead_arr != 0u);
+        const bool is_srv = go & (lead_arr == 0u);
         const bool wake = (key & 3u) == ACT_WAKE_TIME;
         if (TRACE) {
             if (go && pops < a.trace_cap) {
                 a.trace_key[trial * a.trace_cap + pops] = key >> 2;
-                a.trace_time[trial * a.trace_cap + pops] = first_arr ? t_arr : t_srv;
+                a.trace_time[trial * a.trace_cap + pops] = t0;
             }
             pops += go ? 1u : 0u;
         }
-        if (go) now = first_arr ? t_arr : t_srv;        // src/cmb_event.c:239-241
+        if (go) now = t0;                               // src/cmb_event.c:239-241
 
         // ---------------- arrival body (MM1_multi.c:58-66): back from hold -> put
         // Ring accesses are unconditional (a lane that does not put writes its private
@@ -187,11 +195,12 @@ mm1_kernel(const QueueArgs a)
             produced++;
             tail = next_slot(tail);
         }
-        // cmb_objectqueue_put -> cmb_resourceguard_signal(front guard): wake the server
-        if (put & (k_srv == 0u)) {
-            issued++;
-            t_srv = now;
-            k_srv = pack_key(issued, ACT_WAKE_RESOURCE);
+        // cmb_objectqueue_put -> cmb_resourceguard_signal(front guard): wake the server.  The arrival process popped, so
+        // slot 1 is the server's, and it is empty exactly when the server waits at the front guard.
+        if (put & (k1 == 0u)) {
+            last_key += 4u;
+            t1 = now;
+            k1 = last_key | ACT_WAKE_RESOURCE;
         }
 
         // ---------------- service body (MM1_multi.c:78-88)
@@ -213,11 +222,23 @@ mm1_kernel(const QueueArgs a)
         const bool hot = off_next <= ZIG_EXP_MAX * 8u;  // Sfc64::exp_is_hot(u_next)
         const bool push = draw & hot;
         const double when = __dadd_rn(now, __dmul_rn(is_arr ? arr_mean : srv_mean, e_next));
-        if (push) issued++;
-        const double t_new = push ? when : INF;         // the popped slot is refilled or left empty
-        const uint32_t k_new = push ? pack_key(issued, ACT_WAKE_TIME) : 0u;
-        if (is_arr) { t_arr = t_new; k_arr = k_new; }
-        if (is_srv) { t_srv = t_new; k_srv = k_new; }
+        if (push) last_key += 4u;
+        const uint32_t k_new = last_key;
+        // The popped process's next event, if it has one, goes in beside the other pending event (slot 1, the server's
+        // wake-up above included).  Its key is the largest issued so far, so on a tie in time the other goes first, and one
+        // strict compare orders the pair.  A lane that pops either puts its new event ahead or swaps the other one to the
+        // front (with its new event, or none, behind); a lane that does not pop does neither.
+        const bool ahead = push & (when < t1);
+        const bool swap = go & !ahead;
+        const double t_lead = swap ? t1 : (push ? when : t0);
+        const uint32_t k_lead = swap ? k1 : (push ? k_new : k0);
+        if (swap) {
+            t1 = push ? when : INF;
+            k1 = push ? k_new : 0u;
+            lead_arr ^= 1u;                             // the other process leads now
+        }
+        t0 = t_lead;
+        k0 = k_lead;
         if (draw & !hot) flags = is_arr ? 7u : 3u;
         if (push) refill();
 
@@ -247,6 +268,8 @@ mm1_kernel(const QueueArgs a)
             event_step();
         }
         step += MM1_STEPS;
+        wraps += last_key < last_seen ? 1u : 0u;
+        last_seen = last_key;
         if ((step & MM1_PARK_MASK) != 0u) {
             continue;                                   // look at the parked set every (MM1_PARK_MASK+1)-th step only
         }
@@ -258,9 +281,16 @@ mm1_kernel(const QueueArgs a)
                     const bool parked_is_arr = (flags & 4u) != 0u;
                     const double mean = parked_is_arr ? arr_mean : srv_mean;
                     const double at = __dadd_rn(now, __dmul_rn(mean, rng.exp_cold(u_next)));
-                    issued++;
-                    if (parked_is_arr) { t_arr = at; k_arr = pack_key(issued, ACT_WAKE_TIME); }
-                    else               { t_srv = at; k_srv = pack_key(issued, ACT_WAKE_TIME); }
+                    last_key += 4u;
+                    const uint32_t k_at = last_key;
+                    // the parking step left the other process's event (or none) in slot 0 and slot 1 empty: insert
+                    // beside slot 0 as an event step inserts beside slot 1
+                    const bool first = at < t0;
+                    t1 = first ? t0 : at;
+                    k1 = first ? k0 : k_at;
+                    t0 = first ? at : t0;
+                    k0 = first ? k_at : k0;
+                    lead_arr = (first == parked_is_arr) ? 1u : 0u;
                     flags = 1u;
                     refill();
                 }
@@ -268,6 +298,7 @@ mm1_kernel(const QueueArgs a)
         }
     }
     // every update above is predicated on a running lane: the registers hold each trial's results
+    const uint32_t issued = (wraps << 30) + (last_key >> 2);
     if (alive) {
         if (a.events)    a.events[trial] = issued;      // every scheduled event has been popped
         if (a.objects)   a.objects[trial] = served - dropped;
