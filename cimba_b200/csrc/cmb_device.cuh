@@ -405,6 +405,23 @@ enum : uint32_t {
     ACT_CMB_USER = 32u,         // first action id a model may use for its own events (cmb_event_schedule)
 };
 
+// The wildcards of cmb_event_pattern_find / _count / _cancel (include/cmb_event.h:242-255).  An action id is 16 bits in the event
+// list, so ANY_ACTION is no action.  ANY_SUBJECT reserves the subject 0xfffffffe: NIL (the reference's NULL) stays a subject a
+// pattern can name.  An object is stored as 32 bits, so ANY_OBJECT, outside that range, is no object.
+constexpr uint32_t ANY_ACTION = 0xffffffffu;
+constexpr uint32_t ANY_SUBJECT = 0xfffffffeu;
+constexpr int64_t ANY_OBJECT = INT64_MIN;
+
+// Does the pending event (act, subj, arg) match the pattern (pact, psubj, pobj)?  Only the model's own events (act >=
+// ACT_CMB_USER) can: a subject here is a small integer, and a process index would otherwise pass for a subject of the model's
+// choosing - in the reference a model's pattern never matches a process wake-up unless it names the process by its address.
+// The object compares as cmb_event_schedule stores it, in 32 bits.
+CMB_FN bool event_matches(uint32_t act, uint32_t subj, int64_t arg, uint32_t pact, uint32_t psubj, int64_t pobj)
+{
+    return act >= ACT_CMB_USER && (pact == ANY_ACTION || pact == act) && (psubj == ANY_SUBJECT || psubj == subj)
+           && (pobj == ANY_OBJECT || (int32_t)pobj == (int32_t)arg);
+}
+
 // what a process body asks of the dispatcher when it returns (Sim::cmd)
 enum : uint32_t { CMD_NONE = 0u, CMD_HOLD = 1u, CMD_HOLD_EXPONENTIAL = 2u, CMD_GUARD_WAIT = 3u, CMD_EXIT = 4u, CMD_HOLD_SAMPLED = 5u };
 
@@ -714,6 +731,83 @@ struct Sim {
             if (fel.tag[k].subj == subj && fel.tag[k].act < ACT_CMB_USER) hit[m++] = fel.tag[k].key;
         }
         for (uint32_t k = 0u; k < m; k++) (void)event_cancel(hit[k]);
+    }
+
+    // ---------------------------------------------------------------- the event list as a whole, queries (src/cmb_event.c)
+    // cmb_event_queue_initialize(start), :75-82: the clock starts at `start`.  In run_trial before anything is scheduled; a call
+    // after the first schedule flags the trial and leaves the clock where it is.
+    CMB_FN void queue_initialize(double start)
+    {
+        if (fel.issued != 0u) status |= TRIAL_ERR_ARGUMENT;
+        else now = start;
+    }
+
+    CMB_FN bool queue_is_empty() const { return fel.count == 0u; }          // :106-109, process wake-ups included
+    CMB_FN uint64_t queue_count() const { return fel.count; }               // :114-117
+
+    // cmb_event_queue_clear, :97-103 = cmi_hashheap_clear (src/cmi_hashheap.c:153-166): every entry goes, and the key map is off
+    // until the next lookup by key.  Nobody is woken and no key is issued; the issue counter runs on.  Processes stay as they are:
+    // a dropped handle they hold or wait on is "not scheduled" from now on, and its waiter records are dropped with it.  Unlike the
+    // reference's, whose slot 0 is wiped with the rest, cmb_event_current() still names the event being executed.
+    CMB_FN void queue_clear()
+    {
+        fel.count = 0u;
+        fel.map_on = 0u;
+    }
+
+    // cmb_event_time / cmb_event_priority, :155-170.  The reference aborts for a handle that is not scheduled (cmi_hashheap_drank,
+    // src/cmi_hashheap.c:643-656); here the trial is flagged TRIAL_ERR_ARGUMENT and the call returns 0.
+    CMB_FN_NOINLINE double event_time(uint64_t handle)
+    {
+        const uint32_t at = fel.find(arena, handle);
+        if (at == 0u) {
+            status |= TRIAL_ERR_ARGUMENT;
+            return 0.0;
+        }
+        return fel.tag[at].d;
+    }
+
+    CMB_FN_NOINLINE int64_t event_priority(uint64_t handle)
+    {
+        const uint32_t at = fel.find(arena, handle);
+        if (at == 0u) {
+            status |= TRIAL_ERR_ARGUMENT;
+            return 0;
+        }
+        return fel.tag[at].prio;
+    }
+
+    // cmb_event_pattern_find / _count, :351-381 (cmi_hashheap_pattern_find / _count, src/cmi_hashheap.c:741-790): the heap array
+    // from slot 1 up, the model's own events only (event_matches)
+    CMB_FN_NOINLINE uint64_t pattern_find(uint32_t act, uint32_t subj, int64_t obj)
+    {
+        for (uint32_t k = 1u; k <= fel.count; k++) {
+            if (event_matches(fel.tag[k].act, fel.tag[k].subj, fel.tag[k].arg, act, subj, obj)) return fel.tag[k].key;
+        }
+        return 0u;
+    }
+
+    CMB_FN_NOINLINE uint64_t pattern_count(uint32_t act, uint32_t subj, int64_t obj)
+    {
+        uint64_t n = 0u;
+        for (uint32_t k = 1u; k <= fel.count; k++) n += event_matches(fel.tag[k].act, fel.tag[k].subj, fel.tag[k].arg, act, subj, obj) ? 1u : 0u;
+        return n;
+    }
+
+    // cmb_event_pattern_cancel, :385-425: the matches in heap-array order first, then cancelled in that order (their waiters are
+    // woken with CMB_PROCESS_CANCELLED, so the order decides the keys of the wake-ups)
+    CMB_FN_NOINLINE uint64_t pattern_cancel(uint32_t act, uint32_t subj, int64_t obj)
+    {
+        const uint32_t n = (uint32_t)pattern_count(act, subj, obj);
+        if (n == 0u) return 0u;
+        uint64_t *hit = scratch_keys(n);
+        if (hit == nullptr) return 0u;
+        uint32_t m = 0u;
+        for (uint32_t k = 1u; k <= fel.count; k++) {
+            if (event_matches(fel.tag[k].act, fel.tag[k].subj, fel.tag[k].arg, act, subj, obj)) hit[m++] = fel.tag[k].key;
+        }
+        for (uint32_t k = 0u; k < m; k++) (void)event_cancel(hit[k]);
+        return m;
     }
 
     // ---------------------------------------------------------------- processes (src/cmb_process.c)
@@ -1824,6 +1918,21 @@ CMB_FN unsigned dice_faces(S &sim, unsigned n)
 #define cmb_event_reschedule(handle, t)     (sim.event_reschedule((handle), (t)))
 #define cmb_event_reprioritize(handle, pri) (sim.event_reprioritize((handle), (pri)))
 #define cmb_event_is_scheduled(handle)      (sim.event_is_scheduled(handle))
+#define cmb_event_time(handle)              (sim.event_time(handle))
+#define cmb_event_priority(handle)          (sim.event_priority(handle))
+#define cmb_event_queue_initialize(start)   (sim.queue_initialize(start))
+#define cmb_event_queue_is_empty()          (sim.queue_is_empty())
+#define cmb_event_queue_count()             (sim.queue_count())
+#define cmb_event_queue_clear()             (sim.queue_clear())
+// Patterns match the model's own events only (actions >= ACT_CMB_USER), never a process's wake-up; subjects and objects are the
+// values given to cmb_event_schedule.  CMB_ANY_SUBJECT is the subject 0xfffffffe, which a model's events must not use; NULL in
+// the reference is cmb::NIL here, and a pattern may name it.
+#define CMB_ANY_ACTION                      (cimba_b200::cmb::ANY_ACTION)
+#define CMB_ANY_SUBJECT                     (cimba_b200::cmb::ANY_SUBJECT)
+#define CMB_ANY_OBJECT                      (cimba_b200::cmb::ANY_OBJECT)
+#define cmb_event_pattern_find(act, subj, obj)   (sim.pattern_find((act), (subj), (obj)))
+#define cmb_event_pattern_count(act, subj, obj)  (sim.pattern_count((act), (subj), (obj)))
+#define cmb_event_pattern_cancel(act, subj, obj) (sim.pattern_cancel((act), (subj), (obj)))
 #define cmb_objectqueue_initialize(q, cap)  (cimba_b200::cmb::objectqueue_initialize(sim, (q), (cap)))
 #define cmb_objectqueue_length(q)           ((q).length)
 #define cmb_resourcepool_initialize(rp, cap) (cimba_b200::cmb::resourcepool_initialize(sim, (rp), (cap)))

@@ -29,14 +29,15 @@
 // static_fel_high = true;` (StaticSimHigh).
 // A second-form model that also says `static constexpr bool static_waits = true;` (StaticSim<..., PRE = true, W = true>) has
 // cmb_process_timer_add / _timer_cancel / _timers_clear / _timer_set, cmb_process_resume and CMB_PROCESS_YIELD,
-// CMB_PROCESS_WAIT_PROCESS and CMB_PROCESS_WAIT_EVENT, cmb_event_cancel / _reschedule / _reprioritize / _is_scheduled on its own
-// events, and cmb_resourceguard_register with a condition's guard observing another guard: timers, resumes and wake-ups take
+// CMB_PROCESS_WAIT_PROCESS and CMB_PROCESS_WAIT_EVENT, cmb_event_cancel / _reschedule / _reprioritize / _is_scheduled / _time /
+// _priority and cmb_event_pattern_find / _count / _cancel on its own events, and cmb_resourceguard_register with a condition's guard observing another guard: timers, resumes and wake-ups take
 // spare slots, and each process has one wait record.
 // What the tier does NOT have - process creation beyond NPROC; without static_interrupts priorities other than 0, interrupts and
 // pre-emption, and without static_waits timers, resumes, waits on processes and events, events by handle and observers; a process
 // that ends while it holds from two or more containers, or from any without the hook; a queue that outgrows window + ring or its
 // table, a spare slot or a guard heap too few; a cancel of an event somebody waits on by timers_clear, cancel_awaiteds or a stop
-// (whose wake-up order the tier does not keep), a second wait while one is registered - is not an error: the trial is flagged and
+// (whose wake-up order the tier does not keep), a second wait while one is registered, a pattern find with two or more matches or a
+// pattern cancel of two or more events with waiters (both decided by the general engine's heap-array order) - is not an error: the trial is flagged and
 // the launch re-runs it on the general engine from the SAME model template (launch_static_model below), so the answer is the
 // reference's either way.
 //
@@ -48,7 +49,8 @@
 // (test/test_resourcepool.c), coverage_models.cuh's PoolFightT (test/test_resourcepool.c's cast with checks) and
 // tutorial2_model.cuh (tutorial/tut_2_1.c), and with priority queues and conditions guarded_model.cuh (test/test_objectqueue.c,
 // test/test_priorityqueue.c) and coverage_models.cuh's QueueAndTideT; with static_waits coverage_models.cuh's FrontDeskT;
-// examples/tandem_model.cuh; examples/clinic_model.cuh (every cmb_random distribution, alias tables, summaries).
+// examples/tandem_model.cuh; examples/clinic_model.cuh (every cmb_random distribution, alias tables, summaries); with static_waits
+// examples/event_model.cuh (the event list's queries, clear and patterns).
 #pragma once
 
 #include <type_traits>
@@ -838,6 +840,143 @@ struct StaticSim : StaticPriorities<NPROC, PRE>, StaticWaits<NPROC, W> {
         }
         status |= TRIAL_ERR_PROC_OVERFLOW;
         return false;
+    }
+
+    // ---- the event list as a whole (src/cmb_event.c:75-117), as cmb::Sim has it: the clock set before the first schedule, the
+    // occupied slots counted, every slot emptied by a clear.  A clear wakes nobody and issues no key; a wait on a dropped event can
+    // never end, so its record goes (the general engine keeps a record that no lookup finds any more).
+    CMB_FN void queue_initialize(double start)
+    {
+        if (fel.issued != 0u) status |= TRIAL_ERR_ARGUMENT;
+        else now = start;
+    }
+
+    CMB_FN uint64_t queue_count() const
+    {
+        uint64_t n = 0u;
+#pragma unroll
+        for (int i = 0; i < NPROC + NEVENT; i++) n += fel.key[i] != 0u ? 1u : 0u;
+        return n;
+    }
+
+    CMB_FN bool queue_is_empty() const { return queue_count() == 0u; }
+
+    CMB_FN void queue_clear()
+    {
+        const uint32_t issued = fel.issued;
+        fel.clear();
+        fel.issued = issued;
+        if constexpr (W) {
+#pragma unroll
+            for (int i = 0; i < NPROC; i++) {
+                if (this->wkind[i] == this->WAIT_EVENT) this->wkind[i] = this->WAIT_NONE;
+            }
+        }
+    }
+
+    // ---- W: the model's events by handle and by pattern.  cmb_event_time / _priority of a handle that is not pending flag the
+    // trial TRIAL_ERR_ARGUMENT and return 0, as on the general engine.
+    CMB_FN double event_time(uint64_t handle)
+    {
+        double t = 0.0;
+        if constexpr (W) {
+            const int slot = slot_of(handle);
+            if (slot < 0) status |= TRIAL_ERR_ARGUMENT;
+#pragma unroll
+            for (int i = NPROC; i < NPROC + NEVENT; i++) {
+                if (i == slot) t = fel.t[i];
+            }
+        }
+        else {
+            status |= TRIAL_ERR_PROC_OVERFLOW;
+        }
+        return t;
+    }
+
+    CMB_FN int64_t event_priority(uint64_t handle)
+    {
+        int64_t p = 0;
+        if constexpr (W) {
+            const int slot = slot_of(handle);
+            if (slot < 0) status |= TRIAL_ERR_ARGUMENT;
+#pragma unroll
+            for (int i = NPROC; i < NPROC + NEVENT; i++) {
+                if (i == slot) p = fel.prio[i];
+            }
+        }
+        else {
+            status |= TRIAL_ERR_PROC_OVERFLOW;
+        }
+        return p;
+    }
+
+    // the spare slots whose events match the pattern (event_matches: the model's own events only), a bit per slot, and how many
+    CMB_FN uint64_t pattern_slots(uint32_t act, uint32_t subj, int64_t obj, uint64_t &n) const
+    {
+        static_assert(NEVENT <= 64, "a pattern's matches are a 64-bit mask of spare slots");
+        uint64_t hit = 0u;
+        n = 0u;
+#pragma unroll
+        for (int i = 0; i < NEVENT; i++) {
+            if (fel.key[NPROC + i] != 0u && event_matches(uev[i].act, uev[i].subj, uev[i].arg, act, subj, obj)) {
+                hit |= 1ull << i;
+                n++;
+            }
+        }
+        return hit;
+    }
+
+    // cmb_event_pattern_count: the matches, in any order
+    CMB_FN uint64_t pattern_count(uint32_t act, uint32_t subj, int64_t obj)
+    {
+        uint64_t n = 0u;
+        if constexpr (W) (void)pattern_slots(act, subj, obj, n);
+        else status |= TRIAL_ERR_PROC_OVERFLOW;
+        return n;
+    }
+
+    // cmb_event_pattern_find: the general engine returns the first match in its heap array, whose order the tier does not keep -
+    // exact with at most one match; with two or more the trial is flagged
+    CMB_FN uint64_t pattern_find(uint32_t act, uint32_t subj, int64_t obj)
+    {
+        uint64_t handle = 0u;
+        if constexpr (W) {
+            uint64_t n;
+            const uint64_t hit = pattern_slots(act, subj, obj, n);
+            if (n > 1u) status |= TRIAL_ERR_PROC_OVERFLOW;
+#pragma unroll
+            for (int i = 0; i < NEVENT; i++) {
+                if (handle == 0u && ((hit >> i) & 1u) != 0u) handle = fel.key[NPROC + i] >> 2;
+            }
+        }
+        else {
+            status |= TRIAL_ERR_PROC_OVERFLOW;
+        }
+        return handle;
+    }
+
+    // cmb_event_pattern_cancel: every match leaves, and its waiters are woken with CMB_PROCESS_CANCELLED.  The general engine
+    // cancels in heap-array order, so the keys of the wake-ups are exact here only while at most one of the matches has waiters;
+    // with two or more the trial is flagged.
+    CMB_FN uint64_t pattern_cancel(uint32_t act, uint32_t subj, int64_t obj)
+    {
+        if constexpr (W) {
+            uint64_t n;
+            const uint64_t hit = pattern_slots(act, subj, obj, n);
+            int waited = 0;
+#pragma unroll
+            for (int i = 0; i < NEVENT; i++) {
+                if (((hit >> i) & 1u) != 0u && has_waiters(fel.key[NPROC + i] >> 2)) waited++;
+            }
+            if (waited > 1) status |= TRIAL_ERR_PROC_OVERFLOW;
+#pragma unroll
+            for (int i = 0; i < NEVENT; i++) {
+                if (((hit >> i) & 1u) != 0u) (void)event_cancel(fel.key[NPROC + i] >> 2);
+            }
+            return n;
+        }
+        status |= TRIAL_ERR_PROC_OVERFLOW;
+        return 0u;
     }
 
     // cmb_resourceguard_wait up to its yield (src/cmb_resourceguard.c:125-152)

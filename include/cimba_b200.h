@@ -190,7 +190,9 @@ const char *cimba_b200_model_name(int model_id);
 #define CIMBA_B200_TRIAL_NEGATIVE_HOLD  32u
 #define CIMBA_B200_TRIAL_ARENA_EXHAUSTED 64u   /* general engine: a container could not grow (workspace too small) */
 #define CIMBA_B200_TRIAL_BAD_ARGUMENT   128u   /* model code: cmb_random_loaded_dice / _hyperexponential with n = 0, or
-                                                  cmb_random_alias_create with n = 0 or n above the table's capacity */
+                                                  cmb_random_alias_create with n = 0 or n above the table's capacity,
+                                                  cmb_event_time / _priority of an event that is not scheduled (the call
+                                                  returns 0), or cmb_event_queue_initialize after the first schedule */
 
 /* How trials map onto the machine.  LANE: one trial per CUDA thread (32 trials
  * advance per warp instruction; the default for models whose per-trial state is
