@@ -23,6 +23,10 @@ MAP_LANE, MAP_WARP = 1, 32
 
 OK, EINVAL, ENODEVICE, ECUDA, ETRIAL, ENOMEM = 0, -1, -2, -3, -4, -5
 
+# a trial's status word: CIMBA_B200_TRIAL_* bits
+(TRIAL_QUEUE_OVERFLOW, TRIAL_FEL_OVERFLOW, TRIAL_KEY_OVERFLOW, TRIAL_GUARD_OVERFLOW, TRIAL_PROC_OVERFLOW, TRIAL_NEGATIVE_HOLD,
+ TRIAL_ARENA_EXHAUSTED, TRIAL_BAD_ARGUMENT) = 1, 2, 4, 8, 16, 32, 64, 128
+
 
 class DeviceJob(C.Structure):
     """struct cimba_b200_device_job"""

@@ -280,12 +280,13 @@ int launch_kernel(const cimba_b200_device_job *job, void (*plain)(Args), void (*
     return e == cudaSuccess ? CIMBA_B200_OK : cuda_fail(e, what);
 }
 
-// after a fixed-capacity kernel (result e): the general engine re-runs what it flagged, in the arena behind its rings
+// after a fixed-capacity kernel (result e): the general engine re-runs what it flagged, in all of the workspace behind its
+// rings - so a caller whose trials come back CIMBA_B200_TRIAL_ARENA_EXHAUSTED cures that with a larger workspace
 template <class Model>
 int then_repair(int e, const cimba_b200_device_job *job, uint64_t rings_bytes, cudaStream_t st, const char *what)
 {
     if (e != CIMBA_B200_OK || job->status == nullptr) return e;       // nobody could see a flag: nothing to repair by
-    return counted(cmb::launch_repair<Model>(*job, rings_bytes, repair_arena_bytes(job), st), what);
+    return counted(cmb::launch_repair<Model>(*job, rings_bytes, job->workspace_bytes - cmb::align256(rings_bytes), st), what);
 }
 
 // persistent CTAs: as many as are resident at once (`fallback` per SM if the occupancy query fails), at most `wanted`
@@ -1078,6 +1079,75 @@ int cimba_b200_run_experiment(void *array, uint64_t num_trials, size_t stride,
 }
 
 namespace {
+// The trials [lo, hi) of `job` as a job of their own: its arrays offset into the job's, seeds from the global trial index
+cimba_b200_device_job sub_job(const cimba_b200_device_job &job, uint64_t lo, uint64_t hi)
+{
+    cimba_b200_device_job s = job;
+    s.first_trial = job.first_trial + lo;
+    s.num_trials = hi - lo;
+    s.arr_mean = job.arr_mean + lo;
+    s.srv_mean = job.srv_mean + lo;
+    s.events = job.events + lo;
+    s.objects = job.objects + lo;
+    s.t_end = job.t_end + lo;
+    s.sum_wait = job.sum_wait + lo;
+    s.status = job.status + lo;
+    s.max_queue = job.max_queue + lo;
+    s.counters = job.counters + 8u * lo;
+    return s;
+}
+
+// Re-run the trials of `job` whose status (host copy in `status`, kept up to date) says the growth arena ran out.  The
+// arena is shared by every trial of a launch and never reclaimed, so its need grows with the trial count: the run from the
+// first such trial to the last goes again (in one launch; the clean trials in it give what they gave) with 4x the workspace
+// its size asks for, then 4x more per round, up to half of the device's free memory; past that the run is split in halves.  Seeds follow the global trial index, so what comes back
+// is what one launch with room enough would have given.  A trial that still cannot fit keeps its flag.
+int rerun_exhausted(const cimba_b200_device_job &job, uint32_t *status, cudaStream_t st)
+{
+    struct Run { uint64_t lo, hi, ws; };
+    std::vector<Run> todo;
+    auto collect = [&](uint64_t lo, uint64_t hi, uint64_t ws) {     // one run from the first such trial to the last
+        while (lo < hi && (status[lo] & CIMBA_B200_TRIAL_ARENA_EXHAUSTED) == 0u) lo++;
+        while (hi > lo && (status[hi - 1u] & CIMBA_B200_TRIAL_ARENA_EXHAUSTED) == 0u) hi--;
+        if (lo < hi) todo.push_back({lo, hi, ws});
+    };
+    collect(0u, job.num_trials, 0u);
+    while (!todo.empty()) {
+        const Run r = todo.back();
+        todo.pop_back();
+        cimba_b200_device_job s = sub_job(job, r.lo, r.hi);
+        size_t free_bytes = 0, total_bytes = 0;
+        CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
+        const uint64_t cap = free_bytes / 2u;
+        const uint64_t least = cimba_b200_workspace_bytes(&s);
+        uint64_t ws = r.ws != 0u ? r.ws : 4u * least;
+        if (ws > cap) ws = cap;
+        if (ws <= least) continue;                      // no room for more than the first launch had: the flag stays
+        void *mem = nullptr;
+        CUDA_TRY(cudaMalloc(&mem, ws));
+        s.workspace = mem;
+        s.workspace_bytes = ws;
+        int rc = cimba_b200_launch(&s, st);
+        cudaError_t e = cudaSuccess;
+        if (rc == CIMBA_B200_OK) {
+            e = cudaMemcpyAsync(status + r.lo, s.status, (r.hi - r.lo) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        }
+        cudaFree(mem);
+        if (rc != CIMBA_B200_OK) return rc;
+        if (e != cudaSuccess) return cuda_fail(e, "re-run of exhausted trials");
+        if (ws < cap) {
+            collect(r.lo, r.hi, ws < cap / 4u ? 4u * ws : cap);
+        }
+        else if (r.hi - r.lo > 1u) {                    // at the cap: fewer trials share the arena
+            const uint64_t mid = r.lo + (r.hi - r.lo) / 2u;
+            collect(r.lo, mid, cap);
+            collect(mid, r.hi, cap);
+        }
+    }
+    return CIMBA_B200_OK;
+}
+
 int run_experiment_chunk(void *array, uint64_t num_trials, size_t stride, const cimba_b200_experiment *d)
 {
     PhaseClock clk;
@@ -1189,8 +1259,18 @@ int run_experiment_chunk(void *array, uint64_t num_trials, size_t stride, const 
         const uint64_t *ob = ev + n;
         const double *te = (const double *)(ob + n);
         const double *sw = te + n;
-        const uint32_t *stt = (const uint32_t *)(sw + n);
+        uint32_t *stt = (uint32_t *)(sw + n);
         const uint32_t *mq = stt + n;
+        bool exhausted = false;
+        for (uint64_t i = 0; i < n && !exhausted; i++) exhausted = (stt[i] & CIMBA_B200_TRIAL_ARENA_EXHAUSTED) != 0u;
+        if (exhausted) {                                // more workspace for the trials that ran out, then the results again
+            rc = rerun_exhausted(job, stt, st);
+            if (rc != CIMBA_B200_OK) goto done;
+            e = cudaMemcpyAsync(h_out, d_out, out_bytes + (want_counters ? cnt_bytes : 0), cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+            if (e != cudaSuccess) { rc = cuda_fail(e, "D2H after re-run"); goto done; }
+            clk.lap("re-run of exhausted trials");
+        }
         const uint64_t *cnt = (const uint64_t *)(h_out + out_bytes);
         bool any_bad = false;
         for (uint64_t i = 0; i < n; i++) {

@@ -70,10 +70,14 @@ enum : uint32_t {
 // ------------------------------------------------------------------------------------------------ arena
 // Growth memory shared by all trials of a launch: a bump allocator over a slice of the job's workspace.  Blocks a
 // container leaves behind when it doubles are not reused (geometric growth: at most as much again as is live).
+// Every request that does not fit flags the trial (`flag`, its status word, set by Sim::init) - the key map's too, which
+// find() could do without - so a trial runs unflagged exactly when the arena holds all it asks for, and a caller can
+// cure the flag with a larger workspace.
 struct Arena {
     unsigned char *base;
     unsigned long long *cursor;
     unsigned long long bytes;
+    uint32_t *flag = nullptr;
 
     CMB_FN void *alloc(uint64_t n)
     {
@@ -84,7 +88,9 @@ struct Arena {
 #else
         const unsigned long long at = atomicAdd(cursor, (unsigned long long)n);
 #endif
-        return (at + n <= bytes) ? (void *)(base + at) : nullptr;
+        if (at + n <= bytes) return (void *)(base + at);
+        if (flag != nullptr) *flag |= TRIAL_ERR_ARENA;
+        return nullptr;
     }
 };
 
@@ -328,7 +334,7 @@ struct HashHeap {
     CMB_FN_NOINLINE uint32_t find(Arena &arena, uint64_t key)
     {
         if (count == 0u) return 0u;
-        if (!map_activate(arena)) {                    // no room for a map: fall back to scanning
+        if (!map_activate(arena)) {                    // no room for a map (the trial is flagged): fall back to scanning
             for (uint32_t k = 1u; k <= count; k++) {
                 if (tag[k].key == key) return k;
             }
@@ -586,6 +592,7 @@ struct Sim {
         pops = 0u;
         fel_high = 0u;
         arena = a;
+        arena.flag = &status;
         fel.init(fel_store, FEL_INLINE_EXP);
         proc = proc_inline;
         nproc = 0u;

@@ -188,7 +188,8 @@ const char *cimba_b200_model_name(int model_id);
 #define CIMBA_B200_TRIAL_GUARD_OVERFLOW 8u
 #define CIMBA_B200_TRIAL_PROC_OVERFLOW  16u
 #define CIMBA_B200_TRIAL_NEGATIVE_HOLD  32u
-#define CIMBA_B200_TRIAL_ARENA_EXHAUSTED 64u   /* general engine: a container could not grow (workspace too small) */
+#define CIMBA_B200_TRIAL_ARENA_EXHAUSTED 64u   /* general engine: a container could not grow (workspace too small; cimba_b200_launch
+                                                  does not retry - the same job with a larger workspace cures it) */
 #define CIMBA_B200_TRIAL_BAD_ARGUMENT   128u   /* model code: cmb_random_loaded_dice / _hyperexponential with n = 0, or
                                                   cmb_random_alias_create with n = 0 or n above the table's capacity,
                                                   cmb_event_time / _priority of an event that is not scheduled (the call
@@ -343,7 +344,9 @@ typedef struct cimba_b200_experiment {
 } cimba_b200_experiment;
 
 /* Blocks until all trials are done; results written into the caller's array.
- * Returns CIMBA_B200_ETRIAL if any trial's status is non-zero (results of the
+ * Trials that come back CIMBA_B200_TRIAL_ARENA_EXHAUSTED are re-run with more
+ * workspace (up to half of the device's free memory).  Returns
+ * CIMBA_B200_ETRIAL if any trial's status is still non-zero (results of the
  * other trials are still valid). */
 int cimba_b200_run_experiment(void *your_experiment_array,
                               uint64_t num_trials,

@@ -111,10 +111,12 @@ static void run_static(uint64_t seed, const cmb::TrialIn &in, const ZigHot &hot,
 
 // model + 100 = the same model on the static tier (arena_bytes then = entries of the HBM-ring stand-in per queue).
 // model: 0 = MM1, 1 = GG1, 2 = MMC, 3 / 11 / 13 = the guarded queue tests, 5 / 12 = buffer + resource, 14 = test_resource.c, 7 = HOLD, 10 = HARBOR, 16 = RENEGE (the CIMBA_B200_MODEL_* numbers), 17 = examples/tandem_model.cuh, 18 = CHEESE (test/test_resourcepool.c).  arena_bytes of growth memory per call.
-extern "C" int host_cmb_run_trials(int model, int servers, uint64_t master_seed, uint64_t first, uint64_t count,
-                                   uint64_t num_objects, double arr_mean, double srv_mean,
-                                   const double *params, uint32_t num_params, uint64_t arena_bytes,
-                                   uint64_t trace_cap, uint64_t *trace_key, double *trace_time, HostResult *out)
+// arena_used (may be NULL): per trial, the arena cursor when the trial ended - the bytes its containers asked for, granted
+// or not.  Allocation order is fixed by the seed, so a trial runs unflagged exactly when arena_bytes >= that figure.
+static int run_trials(int model, int servers, uint64_t master_seed, uint64_t first, uint64_t count,
+                      uint64_t num_objects, double arr_mean, double srv_mean,
+                      const double *params, uint32_t num_params, uint64_t arena_bytes,
+                      uint64_t trace_cap, uint64_t *trace_key, double *trace_time, HostResult *out, uint64_t *arena_used)
 {
     static ZigHot hot;
     for (int i = 0; i < 256; i++) {
@@ -165,6 +167,27 @@ extern "C" int host_cmb_run_trials(int model, int servers, uint64_t master_seed,
         case 16: run_model<models::Renege>(seed, in, arena, hot, out[i], trace_cap, tk, tt); break;
         default: return -1;
         }
+        if (arena_used) arena_used[i] = cursor;
     }
     return 0;
+}
+
+extern "C" int host_cmb_run_trials(int model, int servers, uint64_t master_seed, uint64_t first, uint64_t count,
+                                   uint64_t num_objects, double arr_mean, double srv_mean,
+                                   const double *params, uint32_t num_params, uint64_t arena_bytes,
+                                   uint64_t trace_cap, uint64_t *trace_key, double *trace_time, HostResult *out)
+{
+    return run_trials(model, servers, master_seed, first, count, num_objects, arr_mean, srv_mean, params, num_params, arena_bytes,
+                      trace_cap, trace_key, trace_time, out, nullptr);
+}
+
+// host_cmb_run_trials + each trial's arena cursor (tests/test_growth_arena.py)
+extern "C" int host_cmb_run_trials_used(int model, int servers, uint64_t master_seed, uint64_t first, uint64_t count,
+                                        uint64_t num_objects, double arr_mean, double srv_mean,
+                                        const double *params, uint32_t num_params, uint64_t arena_bytes,
+                                        uint64_t trace_cap, uint64_t *trace_key, double *trace_time, HostResult *out,
+                                        uint64_t *arena_used)
+{
+    return run_trials(model, servers, master_seed, first, count, num_objects, arr_mean, srv_mean, params, num_params, arena_bytes,
+                      trace_cap, trace_key, trace_time, out, arena_used);
 }
